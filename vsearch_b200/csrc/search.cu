@@ -150,8 +150,9 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
   // post-alignment filter is at its default and no pair can be diverted to the caller's aligner.  VSG_TB_GATE=0 turns
   // it off (A/B runs; the results do not depend on it).
   // VSG_TB_GATE_FORCE=1 (tests): the device takes EVERY leader for accepted, so every follower the replay needs goes
-  // through the re-alignment below
-  bool const tb_force = [] { const char * e = std::getenv("VSG_TB_GATE_FORCE"); return e != nullptr && e[0] == '1'; }();
+  // through the re-alignment below; =2: EVERY leader is rejected, so every follower is walked (and every score-only
+  // checkpoint task re-run with stores, align_ckpt.cuh)
+  int const tb_force = [] { const char * e = std::getenv("VSG_TB_GATE_FORCE"); return e != nullptr && (e[0] == '1' || e[0] == '2') ? e[0] - '0' : 0; }();
   bool tb_gate = false;
   {
     vsg_search_opts d;
@@ -447,7 +448,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
           }
           int const r = align_pairs_gated(c, qset, db, static_cast<int64_t>(hi - lo), Q + lo, T + lo,
                                           o_sc + lo, o_al + lo, o_ma + lo, o_mi + lo, o_ga + lo, o_tr + 4 * lo, nullptr, 0, nullptr,
-                                          lead_part, tb_force ? -1.0 : 100.0 * opt_id + 1e-7, opts->iddef);
+                                          lead_part, tb_force == 1 ? -1.0 : (tb_force == 2 ? 1e9 : 100.0 * opt_id + 1e-7), opts->iddef);
           if (r != VSG_OK) { return r; }
         }
         return VSG_OK;

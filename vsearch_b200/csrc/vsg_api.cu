@@ -276,7 +276,7 @@ extern "C" void vsg_ctx_destroy(vsg_ctx * c)
   if (c->stream != nullptr) { cudaStreamSynchronize(c->stream); }
   for (DevBuf * b : {&c->dir, &c->bnd, &c->he, &c->cigar_scratch, &c->cigar_dense, &c->stats,
                      &c->tasks_fast, &c->tasks_exact, &c->pairs, &c->cigar_len, &c->cigar_offs,
-                     &c->cub_tmp, &c->rank_tmp, &c->rank_scratch, &c->pre_flags, &c->ticket}) { b->release(); }
+                     &c->cub_tmp, &c->rank_tmp, &c->rank_scratch, &c->pre_flags, &c->ticket, &c->rerun_count}) { b->release(); }
   for (PinBuf * b : {&c->h_tasks, &c->h_stats}) { b->release(); }
   for (auto & ev : c->ev) { if (ev != nullptr) { cudaEventDestroy(ev); } }
   for (auto & ev : c->ev_pool) { cudaEventDestroy(ev); }
@@ -473,39 +473,53 @@ void launch_fast(vsg_ctx * c, int R, bool general, bool multi, const DevSeqs & q
 
 // checkpoint forward kernel (align_ckpt.cuh): plain-ACGT tasks use the per-lane profile up to 8 rows per lane and
 // the lane-replicated table above; tasks with IUPAC symbols the 16x16x16 table at 4, 8 or 16 rows per lane
-template <int R, int MODE>
-void launch_ckpt_one(vsg_ctx * c, const DevSeqs & qs, const DevSeqs & ts, const FastTask * d_tasks, int n)
+template <int R, int MODE, int WRITE>
+void launch_ckpt_one(vsg_ctx * c, const DevSeqs & qs, const DevSeqs & ts, const FastTask * d_tasks, int n,
+                     const int32_t * leader_of, int * rerun_count)
 {
   int const blocks = (n + FAST_WARPS - 1) / FAST_WARPS;
   constexpr size_t dyn = ck_dyn_smem(R, MODE);
   if (dyn > 48 * 1024) {
-    cudaFuncSetAttribute(nw_ckpt_kernel<R, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn));
+    cudaFuncSetAttribute(nw_ckpt_kernel<R, MODE, WRITE>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(dyn));
   }
-  nw_ckpt_kernel<R, MODE><<<blocks, FAST_WARPS * 32, dyn, c->stream>>>(
+  nw_ckpt_kernel<R, MODE, WRITE><<<blocks, FAST_WARPS * 32, dyn, c->stream>>>(
       c->sp2, qs, ts, d_tasks, n, static_cast<uint2 *>(c->dir.p), static_cast<uint2 *>(c->bnd.p),
-      static_cast<int32_t *>(c->stats.p));
+      static_cast<int32_t *>(c->stats.p), leader_of, rerun_count);
   count_launch();
 }
 
-void launch_ckpt(vsg_ctx * c, int R, bool general, const DevSeqs & qs, const DevSeqs & ts, const FastTask * d_tasks, int n)
+template <int R, int MODE>
+void launch_ckpt_write(vsg_ctx * c, int write, const DevSeqs & qs, const DevSeqs & ts, const FastTask * d_tasks, int n,
+                       const int32_t * leader_of, int * rerun_count)
+{
+  switch (write) {
+    case CK_SCOREONLY: launch_ckpt_one<R, MODE, CK_SCOREONLY>(c, qs, ts, d_tasks, n, leader_of, rerun_count); break;
+    case CK_RERUN: launch_ckpt_one<R, MODE, CK_RERUN>(c, qs, ts, d_tasks, n, leader_of, rerun_count); break;
+    default: launch_ckpt_one<R, MODE, CK_STORE>(c, qs, ts, d_tasks, n, leader_of, rerun_count); break;
+  }
+}
+
+// write: CK_STORE, CK_SCOREONLY or CK_RERUN (align_ckpt.cuh); leader_of / rerun_count are read by CK_RERUN only
+void launch_ckpt(vsg_ctx * c, int R, bool general, int write, const DevSeqs & qs, const DevSeqs & ts, const FastTask * d_tasks,
+                 int n, const int32_t * leader_of = nullptr, int * rerun_count = nullptr)
 {
   if (general) {
     switch (R) {
-      case 4: launch_ckpt_one<4, CK_GEN>(c, qs, ts, d_tasks, n); break;
-      case 8: launch_ckpt_one<8, CK_GEN>(c, qs, ts, d_tasks, n); break;
-      default: launch_ckpt_one<16, CK_GEN>(c, qs, ts, d_tasks, n); break;
+      case 4: launch_ckpt_write<4, CK_GEN>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); break;
+      case 8: launch_ckpt_write<8, CK_GEN>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); break;
+      default: launch_ckpt_write<16, CK_GEN>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); break;
     }
     return;
   }
   static const bool force_lut = std::getenv("VSG_CK_LUT") != nullptr;   // experiment: table variant (more resident warps) for R <= 8 too
-  if (force_lut && R == 8) { launch_ckpt_one<8, CK_LUT>(c, qs, ts, d_tasks, n); return; }
+  if (force_lut && R == 8) { launch_ckpt_write<8, CK_LUT>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); return; }
   switch (R) {
-#define VSG_CASE(r) case r: launch_ckpt_one<r, CK_PROF>(c, qs, ts, d_tasks, n); break;
+#define VSG_CASE(r) case r: launch_ckpt_write<r, CK_PROF>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); break;
     VSG_CASE(1) VSG_CASE(2) VSG_CASE(3) VSG_CASE(4) VSG_CASE(5) VSG_CASE(6) VSG_CASE(7) VSG_CASE(8)
 #undef VSG_CASE
-#define VSG_CASE(r) case r: launch_ckpt_one<r, CK_LUT>(c, qs, ts, d_tasks, n); break;
+#define VSG_CASE(r) case r: launch_ckpt_write<r, CK_LUT>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); break;
     VSG_CASE(9) VSG_CASE(10) VSG_CASE(11) VSG_CASE(12) VSG_CASE(13) VSG_CASE(14) VSG_CASE(15)
-    default: launch_ckpt_one<16, CK_LUT>(c, qs, ts, d_tasks, n); break;
+    default: launch_ckpt_write<16, CK_LUT>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); break;
 #undef VSG_CASE
   }
 }
@@ -546,7 +560,7 @@ int launch_tb_ckpt_tasks(vsg_ctx * c, int R, bool general, const DevSeqs & qs, c
 }
 
 // A chunk = the tasks whose direction blocks share the scratch buffer at the same time.
-struct ClassRun { int R; bool general, multi, ckpt; size_t first; int count; };  // a run of one kernel class in all_fast
+struct ClassRun { int R; bool general, multi, ckpt, scoreonly; size_t first; int count; };  // a run of one kernel class in all_fast
 struct ChunkPlan {
   std::vector<ClassRun> runs;
   size_t exact_first = 0; int exact_count = 0;
@@ -556,7 +570,8 @@ struct ChunkPlan {
 };
 
 struct ChunkBuilder {  // the chunk being filled
-  std::vector<FastTask> fast[2][3][FAST_RMAX + 1];  // [general][0 = one strip, direction bits; 1 = several strips; 2 = checkpoints][rows per lane]
+  // [general][0 = one strip, direction bits; 1 = several strips; 2 = checkpoints; 3 = checkpoints, score-only][rows per lane]
+  std::vector<FastTask> fast[2][4][FAST_RMAX + 1];
   std::vector<ExactTask> exact;
   uint64_t dir_bytes = 0, bnd_elems = 0, he_elems = 0, cigar_bytes = 0;
   int64_t cells = 0, nfast = 0, nexact = 0;
@@ -625,6 +640,11 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
   const char * const ckpt_min_env = std::getenv("VSG_CKPT_MIN_PAIRS");   // read per call: tests switch it
   int64_t const ckpt_min_pairs = ckpt_min_env != nullptr ? std::atoll(ckpt_min_env) : 2048LL;
   bool const ckpt_any_size = c->ckpt_enabled && npairs >= ckpt_min_pairs;
+  // Traceback on demand (TbGate): a checkpoint task whose pairs are all group followers is usually never walked, so
+  // its forward pass stores no checkpoints (CK_SCOREONLY); the few that phase 2 does walk are recomputed with stores
+  // after phase 1 (CK_RERUN).  VSG_CK_SCOREONLY=0 stores the checkpoints of every task (A/B runs; same results).
+  const char * const so_env = std::getenv("VSG_CK_SCOREONLY");   // read per call: tests switch it
+  bool const scoreonly_ok = leader_of != nullptr && !want_cigar && (so_env == nullptr || so_env[0] != '0');
   std::vector<FastTask> all_fast;
   std::vector<ExactTask> all_exact;
   std::vector<PairDesc> all_pairs;  // CIGAR mode only
@@ -644,15 +664,15 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
   auto close_chunk = [&]() {
     if (cb.empty()) { return; }
     ChunkPlan pl;
-    for (int gm = 0; gm < 6; gm++) {
-      int const g = gm / 3, m = gm % 3;
+    for (int gm = 0; gm < 8; gm++) {
+      int const g = gm / 4, m = gm % 4;
       for (int R = 1; R <= FAST_RMAX; R++) {
         auto & v = cb.fast[g][m][R];
         if (v.empty()) { continue; }
         // longest first: the tail of the grid is made of the short ones
         auto const longer = [](const FastTask & a, const FastTask & b) { return a.dmax > b.dmax; };
         if (!std::is_sorted(v.begin(), v.end(), longer)) { std::sort(v.begin(), v.end(), longer); }
-        pl.runs.push_back(ClassRun{R, g != 0, m == 1, m == 2, all_fast.size(), static_cast<int>(v.size())});
+        pl.runs.push_back(ClassRun{R, g != 0, m == 1, m >= 2, m == 3, all_fast.size(), static_cast<int>(v.size())});
         all_fast.insert(all_fast.end(), v.begin(), v.end());
         v.clear();
       }
@@ -761,7 +781,8 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
         if (pair2) { add_pairdesc(q, b.t, ck ? 2 : 0, b.slot, R, ck ? (gbit | 1) : 1, dmax, ft.dir_off, ft.bnd_off); }
         cb.dir_bytes += align_up(dirb, 32);
         cb.bnd_elems += auxe;
-        cb.fast[a.general ? 1 : 0][ck ? 2 : (ns > 1 ? 1 : 0)][R].push_back(ft);
+        bool const scoreonly = ck && scoreonly_ok && leader_of[a.slot] >= 0 && (!pair2 || leader_of[b.slot] >= 0);
+        cb.fast[a.general ? 1 : 0][scoreonly ? 3 : (ck ? 2 : (ns > 1 ? 1 : 0))][R].push_back(ft);
         cb.cells += static_cast<int64_t>(Q) * a.d + (pair2 ? static_cast<int64_t>(Q) * b.d : 0);
         cb.nfast += pair2 ? 2 : 1;
         k += pair2 ? 2 : 1;
@@ -844,6 +865,19 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
     c->ev_pool.push_back(e);
   }
 
+  // VSG_TRACE: how many checkpoint tasks stored their checkpoints, ran score-only, and were re-run with stores
+  int64_t n_stored = 0, n_scoreonly = 0;
+  int * d_rerun = nullptr;
+  if (trace) {
+    for (auto const & pl : plans) {
+      for (auto const & run : pl.runs) { if (run.ckpt) { (run.scoreonly ? n_scoreonly : n_stored) += run.count; } }
+    }
+    if (n_scoreonly > 0) {
+      if ((rc = c->rerun_count.reserve(64)) != VSG_OK) { return rc; }
+      d_rerun = static_cast<int *>(c->rerun_count.p);
+      VSG_CUDA_OK(cudaMemsetAsync(d_rerun, 0, sizeof(int), c->stream));
+    }
+  }
   FastTask * const d_fast = static_cast<FastTask *>(c->tasks_fast.p);
   ExactTask * const d_exact = static_cast<ExactTask *>(c->tasks_exact.p);
   int32_t * const d_stats = static_cast<int32_t *>(c->stats.p);
@@ -853,7 +887,7 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
     ChunkPlan const & pl = plans[ci];
     VSG_CUDA_OK(cudaEventRecord(c->ev_pool[3 * ci], c->stream));
     for (auto const & run : pl.runs) {
-      if (run.ckpt) { launch_ckpt(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count); }
+      if (run.ckpt) { launch_ckpt(c, run.R, run.general, run.scoreonly ? CK_SCOREONLY : CK_STORE, queries->d, targets->d, d_fast + run.first, run.count); }
       else { launch_fast(c, run.R, run.general, run.multi, queries->d, targets->d, d_fast + run.first, run.count); }
     }
     if (pl.exact_count > 0) {
@@ -872,6 +906,12 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
           GateRun const & g = gate_runs[ci][ri];
           TbGate const g1{d_gate_ids + g.lead_first, static_cast<int>(g.lead_count), d_leader, 1, gate_iddef, gate_threshold};
           if ((rc = launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, g1)) != VSG_OK) { return rc; }
+        }
+        // the checkpoints of the score-only tasks phase 2 will walk (a follower whose leader was not accepted)
+        for (auto const & run : pl.runs) {
+          if (run.scoreonly) {
+            launch_ckpt(c, run.R, run.general, CK_RERUN, queries->d, targets->d, d_fast + run.first, run.count, d_leader, d_rerun);
+          }
         }
       }
       for (size_t ri = 0; ri < pl.runs.size(); ri++) {
@@ -953,6 +993,8 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
       for (int p = 0; p < np; p++) { cigars[static_cast<size_t>(hpairs[p].out)] = std::string(dense.data() + h_offs[static_cast<size_t>(p)]); }
     }
   }
+  int h_rerun = 0;
+  if (d_rerun != nullptr) { VSG_CUDA_OK(cudaMemcpyAsync(&h_rerun, d_rerun, sizeof(int), cudaMemcpyDeviceToHost, c->stream)); }
   if (!plans.empty()) {
     VSG_CUDA_OK(cudaMemcpyAsync(hs, d_stats, sizeof(int32_t) * VSG_STAT_WORDS * static_cast<size_t>(npairs), cudaMemcpyDeviceToHost, c->stream));
   }
@@ -998,6 +1040,10 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
                  static_cast<long long>(npairs), plans.size(),
                  std::chrono::duration<double, std::milli>(t_planned - t_begin).count(),
                  std::chrono::duration<double, std::milli>(t_end - t_begin).count());
+    if (n_stored + n_scoreonly > 0) {
+      std::fprintf(stderr, "[vsg trace] align_pairs checkpoint tasks: %lld stored, %lld score-only, %d of them re-run with stores\n",
+                   static_cast<long long>(n_stored), static_cast<long long>(n_scoreonly), h_rerun);
+    }
   }
   return VSG_OK;
 }

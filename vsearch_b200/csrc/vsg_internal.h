@@ -131,7 +131,7 @@ struct vsg_ctx {
   bool fast_disabled = false;  // VSG_DISABLE_FAST=1 (tests force the exact kernel)
   // scratch
   vsg::DevBuf dir, bnd, he, cigar_scratch, cigar_dense, stats, tasks_fast, tasks_exact, pairs,
-      cigar_len, cigar_offs, cub_tmp, rank_tmp, rank_scratch, pre_flags, ticket, gate;
+      cigar_len, cigar_offs, cub_tmp, rank_tmp, rank_scratch, pre_flags, ticket, gate, rerun_count;
   vsg::PinBuf h_tasks, h_stats;
   size_t dir_budget = (size_t)64 << 30;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
