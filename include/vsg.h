@@ -113,6 +113,18 @@ int vsg_align_pairs(vsg_ctx * ctx, const vsg_seqset * queries, const vsg_seqset 
                     uint16_t * mismatches, uint16_t * gaps, int32_t * trims,
                     char * cigar_buf, int64_t cigar_cap, int64_t * cigar_off);
 
+/* vsg_align_pairs (statistics only) with traceback on demand, as vsg_search_batch calls it.  For tools/tests.
+ *      leader_of[i] = -1 for a group leader or an ungated pair, else the index in this call of pair i's leader,
+ *      which must itself have -1 (VSG_EINVAL otherwise).  A follower whose leader passes the identity test
+ *      (threshold = 100 * id + margin, under iddef) may come back "not computed": aligned = matches = mismatches =
+ *      0xffff, trims and gaps unspecified; its score is always computed.  ck_counts (optional, 3 x int64): checkpoint
+ *      tasks that stored their checkpoints, that ran score-only, and the score-only ones re-run with stores. */
+int vsg_align_pairs_gated(vsg_ctx * ctx, const vsg_seqset * queries, const vsg_seqset * targets,
+                          int64_t npairs, const uint32_t * qidx, const uint32_t * tidx,
+                          int16_t * score, uint16_t * aligned, uint16_t * matches,
+                          uint16_t * mismatches, uint16_t * gaps, int32_t * trims,
+                          const int32_t * leader_of, double threshold, int iddef, int64_t * ck_counts);
+
 /* Layout of the per-pair statistics record the kernels produce (8 x int32, device side);
  * exposed so that tools reading the raw buffers agree on it. */
 #define VSG_STAT_SCORE 0
@@ -139,6 +151,8 @@ typedef struct vsg_profile {
   float rank_ms;
   float reserved;
   int64_t tb_skipped;   /* pairs whose walk back was skipped by traceback on demand (vsg_search_batch; their DP was computed) */
+  int64_t tb_redone;    /* skipped pairs vsg_search_batch needed after all and re-aligned one by one: the device's verdict
+                           on their group leader differed from the host's (only a borderline identity can do that) */
 } vsg_profile;
 int vsg_profile_reset(vsg_ctx * ctx);
 int vsg_profile_get(vsg_ctx * ctx, vsg_profile * out);

@@ -8,6 +8,7 @@ import ctypes as C
 import hashlib
 import json
 import os
+import re
 import subprocess
 
 import numpy as np
@@ -348,3 +349,83 @@ class RefDb:
                              int(al[o]), int(acc[o]), int(st[o])))
             out.append(rows)
         return out
+
+
+def trims_from_cigar(c):
+    """(trim_q_left, trim_t_left, trim_q_right, trim_t_right): run length of a leading / trailing D resp. I"""
+    ops = re.findall(r"(\d*)([MID])", c)
+    if not ops:
+        return (0, 0, 0, 0)
+    f, l = ops[0], ops[-1]
+    fr = int(f[0]) if f[0] else 1
+    lr = int(l[0]) if l[0] else 1
+    return (fr if f[1] == "D" else 0, fr if f[1] == "I" else 0,
+            lr if l[1] == "D" else 0, lr if l[1] == "I" else 0)
+
+
+def finish_hit(qlen, tlen, aligned, matches, mismatches, gaps, trims, iddef):
+    """align_trim and the identity definitions (searchcore.cpp:409-463) in float64, the host's finish_hit restated:
+    (internal_alignment_length, internal_gaps, id under iddef)"""
+    tql, ttl, tqr, ttr = trims
+    if tql >= aligned:
+        tqr = 0
+    if ttl >= aligned:
+        ttr = 0
+    internal = aligned - (tql + ttl + tqr + ttr)
+    internal_gaps = gaps - (1 if tql + ttl > 0 else 0) - (1 if tqr + ttr > 0 else 0)
+    shortest, longest = min(qlen, tlen), max(qlen, tlen)
+    if iddef == 0:
+        ident = 100.0 * matches / shortest if shortest > 0 else 0.0
+    elif iddef == 2:
+        ident = 100.0 * matches / internal if internal > 0 else 0.0
+    elif iddef == 3:
+        ident = max(0.0, 100.0 * (1.0 - (1.0 * (mismatches + gaps) / longest)))
+    else:                                                     # 1 and 4
+        ident = 100.0 * matches / aligned if aligned > 0 else 0.0
+    return internal, internal_gaps, ident
+
+
+def leader_accepted(qlen, tlen, aligned, matches, mismatches, gaps, trims, iddef, threshold):
+    """the device's verdict on a group leader (align_ckpt.cuh tb_leader_accepted) restated: the identity test of
+    search_acceptable_aligned with every optional filter at its default"""
+    return matches > 0 and finish_hit(qlen, tlen, aligned, matches, mismatches, gaps, trims, iddef)[2] >= threshold
+
+
+def oracle_row_fields(q: bytes, t: bytes, iddef=2, pen=None, n_mismatch=0):
+    """what a search result row for (q, t) holds according to the oracle: score and statistics of oracle_nw16, the
+    trims of its CIGAR and finish_hit's internal length, internal gaps and identity"""
+    score, al, ma, mi, ga, cig = oracle_nw16(q, t, pen, n_mismatch)
+    trims = trims_from_cigar(cig)
+    internal, igaps, ident = finish_hit(len(q), len(t), al, ma, mi, ga, trims, iddef)
+    return dict(nwscore=score, aligned=al, matches=ma, mismatches=mi, gaps=ga, trims=trims,
+                internal_alignment_length=internal, internal_gaps=igaps, id=ident)
+
+
+ROW_FIELDS = ("nwscore", "query_length", "target_length", "matches", "mismatches", "gaps", "alignment_length",
+              "internal_alignment_length", "internal_gaps", "id")
+
+
+def check_search_rows(res, counts, max_results, queries, targets, iddef=2, pen=None, n_mismatch=0):
+    """every returned row of a plus-strand search against the oracle, field by field (nwscore, lengths, statistics,
+    internal alignment length and gaps, identity).  queries / targets: synth.SeqSet or lists of bytes.
+    Returns the number of rows checked."""
+    seq_q = queries.seq if hasattr(queries, "seq") else queries.__getitem__
+    seq_t = targets.seq if hasattr(targets, "seq") else targets.__getitem__
+    bad, n = [], 0
+    cache = {}
+    for i in range(len(counts)):
+        for j in range(int(counts[i])):
+            r = res[i * max_results + j]
+            assert r.strand == 0, (i, j)
+            key = (i, r.target)
+            if key not in cache:
+                q, t = seq_q(i), seq_t(r.target)
+                o = oracle_row_fields(q, t, iddef, pen, n_mismatch)
+                cache[key] = (o["nwscore"], len(q), len(t), o["matches"], o["mismatches"], o["gaps"], o["aligned"],
+                              o["internal_alignment_length"], o["internal_gaps"], o["id"])
+            got = tuple(getattr(r, f) for f in ROW_FIELDS)
+            if got != cache[key]:
+                bad.append((i, j, r.target, dict(zip(ROW_FIELDS, got)), dict(zip(ROW_FIELDS, cache[key]))))
+            n += 1
+    assert not bad, f"{len(bad)} of {n} rows differ from the oracle; first: {bad[:2]}"
+    return n

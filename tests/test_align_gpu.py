@@ -1,7 +1,6 @@
 """GPU parity tests of the batched aligner (vsg_align_pairs) against the oracle.
 Bit-exact on score, alignment statistics and CIGAR (integer/byte work: no tolerance)."""
 import os
-import re
 
 import numpy as np
 import pytest
@@ -20,15 +19,7 @@ def rand_seq(rng, n, alphabet=b"ACGT"):
     return a[rng.integers(0, a.shape[0], size=n)].tobytes()
 
 
-def trims_from_cigar(c):
-    ops = re.findall(r"(\d*)([MID])", c)
-    if not ops:
-        return (0, 0, 0, 0)
-    f, l = ops[0], ops[-1]
-    fr = int(f[0]) if f[0] else 1
-    lr = int(l[0]) if l[0] else 1
-    return (fr if f[1] == "D" else 0, fr if f[1] == "I" else 0,
-            lr if l[1] == "D" else 0, lr if l[1] == "I" else 0)
+trims_from_cigar = checkers.trims_from_cigar
 
 
 def check(ctx, qseqs, tseqs, pairs, pen=None, n_mismatch=0, expect_kernel=None):

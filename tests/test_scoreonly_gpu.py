@@ -59,6 +59,8 @@ def test_scoreonly_tasks_do_not_change_the_hit_tables(maxaccepts, ident):
                 with env(**case):
                     res, counts, work = ctx.search(ix, db, qs, 0, len(qss), o, th)
                 assert checkers.digest([rows_of(res, counts, i, th) for i in range(len(qss))]) == want, case
+                # nwscore included: a follower's score comes from the score-only pass
+                assert checkers.check_search_rows(res, counts, th, qss, dbs) > 0, case
     finally:
         ix.close(); db.close(); qs.close()
         ctx.close()

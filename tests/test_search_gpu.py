@@ -73,6 +73,8 @@ def test_rank_and_search_golden(ctx):
                 assert [r[1] for r in got] == sorted([r[1] for r in got], reverse=True)
             else:
                 assert got == want, (case["id"], i, got, want)
+        if not case["strand_both"]:
+            checkers.check_search_rows(res, counts, th, qss, dbs)
         assert work[0] > 0 and work[1] > 0
         # the default run above took the "tail" shortcut at once (few queries: all remaining candidates
         # in one device call); without it the driver aligns exactly the reference's pairs
@@ -207,6 +209,7 @@ def test_search_vs_compiled_reference(ctx):
         assert got == [list(t) for t in want[i]], i
         hit += bool(got) and got[0][0] == int(src[i])
     assert hit > 100
+    checkers.check_search_rows(res, counts, th, qss, dbs)
     ol = gpu_opts(0.9, 1, 32); ol.lazy = 1
     with no_tail():
         res2, counts2, work2 = ctx.search(ix, db, qs, 0, len(qss), ol, th)
@@ -252,6 +255,7 @@ def test_traceback_on_demand_does_not_change_the_hit_tables(ctx, maxaccepts, ide
                 for k in env:
                     del os.environ[k]
             assert checkers.digest([rows_of(res, counts, i, th) for i in range(len(qss))]) == want, env
+            assert checkers.check_search_rows(res, counts, th, qss, dbs) > 0, env
     finally:
         del os.environ["VSG_CKPT_MIN_PAIRS"]
     ix.close(); db.close(); qs.close()
@@ -380,4 +384,63 @@ def test_optional_filters_vs_compiled_reference(ctx):
             assert got == [list(t) for t in want[i]], (case, i)
             nrows += len(got)
         assert nrows > 0, case
+        checkers.check_search_rows(res, counts, th, qss, dbs)
     ix.close(); db.close(); qs.close()
+
+
+@pytest.mark.parametrize("iddef", [0, 1, 3, 4])
+def test_gated_search_vs_oracle_every_field(iddef):
+    """traceback on demand under every other --iddef, with a non-default scoring and queries of 300 to 500 nt (the
+    table and IUPAC checkpoint kernels): whole rows, nwscore included, equal the oracle's, with the device's verdicts
+    as they are and with every leader rejected (every follower walked from re-run checkpoints).  No skipped walk may
+    be needed by the replay: the device's verdict on every leader is the host's."""
+    rng = np.random.default_rng(61 + iddef)
+    pen = np.array([1, -2, 3, 3, 10, 10, 3, 3, 1, 1, 1, 1, 1, 1], dtype=np.int64)
+    # families of five 2-10 % variants: every query has several candidates, the group followers.  Queries are whole
+    # variants, so that identities over the whole alignment (iddef 1, 3, 4) reach the threshold too
+    roots = [synth.random_seqs(rng, 1, int(rng.integers(300, 501)))[0] for _ in range(60)]
+    seqs = [synth.mutate(rng, roots[i // 5], float(rng.uniform(0.02, 0.1))) for i in range(300)]
+    queries = []
+    for i in range(48):
+        q = synth.mutate(rng, seqs[int(rng.integers(0, 300))], 0.05 if i % 2 else 0.01)
+        if i % 3 == 0:
+            q[int(rng.integers(0, q.shape[0]))] = ord("N")
+        queries.append(q.tobytes())
+    dbs = synth.SeqSet(seqs); qss = synth.SeqSet(queries)
+    # weak_id 0.8: rejected candidates at 80 % or more are listed too, followers walked after a rejected leader among them
+    opts = checkers.search_opts(len(dbs), id=0.97, maxaccepts=1, maxrejects=8, iddef=iddef, weak_id=0.8)
+    od = checkers.OracleDb(dbs)
+    want = [[[h.target, h.id, h.matches, h.mismatches, h.nwgaps, h.nwalignmentlength, h.accepted, h.strand, h.nwscore,
+              h.internal_alignmentlength, h.internal_gaps] for h in od.search(q, opts, pen)[0]] for q in queries]
+    od.close()
+    assert sum(len(w) for w in want) > 100
+    ctx = vlib.Context(0, pen=pen)
+    db = ctx.seqset(dbs); qs = ctx.seqset(qss)
+    ix = ctx.index(db, 8, 0)
+    o = gpu_opts(0.97, 1, 8); o.iddef = iddef; o.weak_id = 0.8
+    try:
+        for case in ({}, {"VSG_TB_GATE_FORCE": "2"}):
+            kv = dict(case, VSG_CKPT_MIN_PAIRS="0")
+            old = {k: os.environ.get(k) for k in kv}
+            os.environ.update(kv)
+            try:
+                with no_tail():
+                    ctx.profile_reset()
+                    res, counts, _ = ctx.search(ix, db, qs, 0, len(queries), o, opts.tophits)
+                    prof = ctx.profile()
+            finally:
+                for k, v in old.items():
+                    if v is None:
+                        del os.environ[k]
+                    else:
+                        os.environ[k] = v
+            for i in range(len(queries)):
+                got = [[r.target, r.id, r.matches, r.mismatches, r.gaps, r.alignment_length, r.accepted, r.strand, r.nwscore,
+                        r.internal_alignment_length, r.internal_gaps]
+                       for r in (res[i * opts.tophits + j] for j in range(int(counts[i])))]
+                assert got == want[i], (case, i)
+            checkers.check_search_rows(res, counts, opts.tophits, qss, dbs, iddef=iddef, pen=pen)
+            assert prof.tb_redone == 0, case
+            assert (prof.tb_skipped > 0) == (not case), (case, prof.tb_skipped)
+    finally:
+        ix.close(); db.close(); qs.close(); ctx.close()

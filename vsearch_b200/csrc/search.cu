@@ -631,6 +631,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
     }
     t_join += ms(tp0, now());
   }
+  c->prof_tb_redone += tb_redone;
   if (trace) {
     std::fprintf(stderr, "[vsg trace] batch@%lld: rank %.1f init %.1f gather %.1f align %.1f replay %.1f join %.1f ms; done at %.1f ms; %lld skipped walks redone\n",
                  static_cast<long long>(b0), t_rank, t_init, t_gather, t_align, t_replay, t_join, ms(t_call0, now()), static_cast<long long>(tb_redone));
@@ -669,7 +670,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
   for (int t = 0; t < nthreads; t++) {
     vsg_ctx * wc = c->children[static_cast<size_t>(t)];
     c->prof_cells += wc->prof_cells; c->prof_fast += wc->prof_fast; c->prof_exact += wc->prof_exact;
-    c->prof_tb_skipped += wc->prof_tb_skipped;
+    c->prof_tb_skipped += wc->prof_tb_skipped; c->prof_tb_redone += wc->prof_tb_redone;
     c->prof_fwd_launches += wc->prof_fwd_launches;
     c->prof_fwd_ms += wc->prof_fwd_ms; c->prof_tb_ms += wc->prof_tb_ms; c->prof_rank_ms += wc->prof_rank_ms;
     vsg_profile_reset(wc);

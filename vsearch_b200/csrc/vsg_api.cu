@@ -593,6 +593,28 @@ extern "C" int vsg_align_pairs(vsg_ctx * c, const vsg_seqset * queries, const vs
                                 cigar_buf, cigar_cap, cigar_off, nullptr, 0.0, 2);
 }
 
+extern "C" int vsg_align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_seqset * targets,
+                                     int64_t npairs, const uint32_t * qidx, const uint32_t * tidx,
+                                     int16_t * score, uint16_t * aligned, uint16_t * matches,
+                                     uint16_t * mismatches, uint16_t * gaps, int32_t * trims,
+                                     const int32_t * leader_of, double threshold, int iddef, int64_t * ck_counts)
+{
+  if (npairs > 0 && leader_of == nullptr) { Error::set("vsg_align_pairs_gated: leader_of required"); return VSG_EINVAL; }
+  if (ck_counts != nullptr) { ck_counts[0] = ck_counts[1] = ck_counts[2] = 0; }
+  // the kernels read the verdict of leader_of[k] from its statistics record: a leader in this call that is not
+  // itself a follower
+  for (int64_t k = 0; k < npairs; k++) {
+    int32_t const l = leader_of[k];
+    if (l != -1 && (l < 0 || l >= npairs || leader_of[l] != -1)) {
+      Error::set("vsg_align_pairs_gated: leader_of[" + std::to_string(k) + "] = " + std::to_string(l) +
+                 " is neither -1 nor the index of a leader in this call");
+      return VSG_EINVAL;
+    }
+  }
+  return vsg::align_pairs_gated(c, queries, targets, npairs, qidx, tidx, score, aligned, matches, mismatches, gaps, trims,
+                                nullptr, 0, nullptr, leader_of, threshold, iddef, ck_counts);
+}
+
 // leader_of (optional, npairs entries, statistics-only calls): traceback on demand, see align_ckpt.cuh (TbGate).  A pair
 // whose walk was skipped comes back with aligned = matches = mismatches = 0xffff.
 int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_seqset * targets,
@@ -600,7 +622,7 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
                            int16_t * score, uint16_t * aligned, uint16_t * matches,
                            uint16_t * mismatches, uint16_t * gaps, int32_t * trims,
                            char * cigar_buf, int64_t cigar_cap, int64_t * cigar_off,
-                           const int32_t * leader_of, double gate_threshold, int gate_iddef)
+                           const int32_t * leader_of, double gate_threshold, int gate_iddef, int64_t * ck_counts)
 {
   if (c == nullptr || queries == nullptr || targets == nullptr || npairs < 0 ||
       (npairs > 0 && (qidx == nullptr || tidx == nullptr || score == nullptr))) {
@@ -865,10 +887,10 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
     c->ev_pool.push_back(e);
   }
 
-  // VSG_TRACE: how many checkpoint tasks stored their checkpoints, ran score-only, and were re-run with stores
+  // VSG_TRACE and ck_counts: how many checkpoint tasks stored their checkpoints, ran score-only, and were re-run with stores
   int64_t n_stored = 0, n_scoreonly = 0;
   int * d_rerun = nullptr;
-  if (trace) {
+  if (trace || ck_counts != nullptr) {
     for (auto const & pl : plans) {
       for (auto const & run : pl.runs) { if (run.ckpt) { (run.scoreonly ? n_scoreonly : n_stored) += run.count; } }
     }
@@ -1034,6 +1056,7 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
     }
   }
   if (want_cigar) { cigar_off[npairs] = cpos; }
+  if (ck_counts != nullptr) { ck_counts[0] = n_stored; ck_counts[1] = n_scoreonly; ck_counts[2] = h_rerun; }
   if (trace) {
     auto const t_end = std::chrono::steady_clock::now();
     std::fprintf(stderr, "[vsg trace] align_pairs %lld pairs, %zu chunk(s): plan %.1f ms, total %.1f ms\n",
@@ -1103,7 +1126,7 @@ extern "C" int vsg_measure_int_peak(vsg_ctx * c, double * packed_lane_ops_per_s)
 extern "C" int vsg_profile_reset(vsg_ctx * c)
 {
   if (c == nullptr) { return VSG_EINVAL; }
-  c->prof_cells = c->prof_fast = c->prof_exact = c->prof_fwd_launches = c->prof_tb_skipped = 0;
+  c->prof_cells = c->prof_fast = c->prof_exact = c->prof_fwd_launches = c->prof_tb_skipped = c->prof_tb_redone = 0;
   c->prof_fwd_ms = c->prof_tb_ms = c->prof_rank_ms = 0.f;
   return VSG_OK;
 }
@@ -1116,5 +1139,6 @@ extern "C" int vsg_profile_get(vsg_ctx * c, vsg_profile * out)
   out->fwd_ms = c->prof_fwd_ms; out->traceback_ms = c->prof_tb_ms; out->rank_ms = c->prof_rank_ms;
   out->reserved = 0.f;
   out->tb_skipped = c->prof_tb_skipped;
+  out->tb_redone = c->prof_tb_redone;
   return VSG_OK;
 }

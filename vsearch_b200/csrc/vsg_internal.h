@@ -101,13 +101,14 @@ struct PinBuf {
 void count_launch(int n = 1);
 
 // vsg_align_pairs with traceback on demand (align_ckpt.cuh, TbGate): leader_of[k] = index of pair k's group leader in
-// this call, or -1; threshold = 100 * --id (+ margin); skipped pairs return aligned = matches = mismatches = 0xffff
+// this call, or -1; threshold = 100 * --id (+ margin); skipped pairs return aligned = matches = mismatches = 0xffff.
+// ck_counts (optional, 3 entries): checkpoint tasks stored, score-only, re-run with stores
 int align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_seqset * targets,
                       int64_t npairs, const uint32_t * qidx, const uint32_t * tidx,
                       int16_t * score, uint16_t * aligned, uint16_t * matches,
                       uint16_t * mismatches, uint16_t * gaps, int32_t * trims,
                       char * cigar_buf, int64_t cigar_cap, int64_t * cigar_off,
-                      const int32_t * leader_of, double gate_threshold, int gate_iddef);
+                      const int32_t * leader_of, double gate_threshold, int gate_iddef, int64_t * ck_counts = nullptr);
 
 }  // namespace vsg
 
@@ -136,7 +137,7 @@ struct vsg_ctx {
   size_t dir_budget = (size_t)64 << 30;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   // cumulative profile since the last vsg_profile_reset (kernel times from cudaEvents on `stream`)
-  int64_t prof_cells = 0, prof_fast = 0, prof_exact = 0, prof_fwd_launches = 0, prof_tb_skipped = 0;
+  int64_t prof_cells = 0, prof_fast = 0, prof_exact = 0, prof_fwd_launches = 0, prof_tb_skipped = 0, prof_tb_redone = 0;
   float prof_fwd_ms = 0.f, prof_tb_ms = 0.f, prof_rank_ms = 0.f;
   bool rank_pending = false;
   std::vector<cudaEvent_t> ev_pool;  // 3 per chunk of an align call

@@ -51,7 +51,7 @@ class SearchOpts(C.Structure):
 class Profile(C.Structure):
     _fields_ = [("cells", C.c_int64), ("fast_pairs", C.c_int64), ("exact_pairs", C.c_int64),
                 ("fwd_launches", C.c_int64), ("fwd_ms", C.c_float), ("traceback_ms", C.c_float),
-                ("rank_ms", C.c_float), ("reserved", C.c_float), ("tb_skipped", C.c_int64)]
+                ("rank_ms", C.c_float), ("reserved", C.c_float), ("tb_skipped", C.c_int64), ("tb_redone", C.c_int64)]
 
 
 class SearchResult(C.Structure):
@@ -263,6 +263,31 @@ class Context:
         pr = self.profile()
         return AlignResult(score, al, ma, mi, ga, trims, cigs, pr.cells, pr.fwd_ms, pr.traceback_ms,
                            pr.fast_pairs, pr.exact_pairs)
+
+    def align_pairs_gated(self, qs: SeqSetHandle, ts: SeqSetHandle, qidx: np.ndarray, tidx: np.ndarray,
+                          leader_of: np.ndarray, threshold: float, iddef: int):
+        """vsg_align_pairs_gated -> (AlignResult, (stored, score-only, re-run) checkpoint task counts, tb_skipped)"""
+        lib = load()
+        qidx = np.ascontiguousarray(qidx, dtype=np.uint32)
+        tidx = np.ascontiguousarray(tidx, dtype=np.uint32)
+        lead = np.ascontiguousarray(leader_of, dtype=np.int32)
+        n = int(qidx.shape[0])
+        assert tidx.shape[0] == n and lead.shape[0] == n
+        score = np.zeros(n, dtype=np.int16)
+        al = np.zeros(n, dtype=np.uint16); ma = np.zeros(n, dtype=np.uint16)
+        mi = np.zeros(n, dtype=np.uint16); ga = np.zeros(n, dtype=np.uint16)
+        trims = np.zeros((n, 4), dtype=np.int32)
+        ck = np.zeros(3, dtype=np.int64)
+        self.profile_reset()
+        _check(lib.vsg_align_pairs_gated(self.h, qs.h, ts.h, C.c_int64(n), _ptr(qidx, C.c_uint32), _ptr(tidx, C.c_uint32),
+                                         _ptr(score, C.c_int16), _ptr(al, C.c_uint16), _ptr(ma, C.c_uint16),
+                                         _ptr(mi, C.c_uint16), _ptr(ga, C.c_uint16), _ptr(trims, C.c_int32),
+                                         _ptr(lead, C.c_int32), C.c_double(threshold), C.c_int(iddef),
+                                         _ptr(ck, C.c_int64)), "vsg_align_pairs_gated")
+        pr = self.profile()
+        res = AlignResult(score, al, ma, mi, ga, trims, None, pr.cells, pr.fwd_ms, pr.traceback_ms,
+                          pr.fast_pairs, pr.exact_pairs)
+        return res, tuple(int(x) for x in ck), int(pr.tb_skipped)
 
     def index(self, db: SeqSetHandle, wordlength: int = 8, mask_lower: int = 0) -> IndexHandle:
         h = C.c_void_p()
