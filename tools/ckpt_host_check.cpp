@@ -147,8 +147,8 @@ int main(int argc, char ** argv)
       for (int x = 0; x < D; x++) { ts[h][x] = (k % 2 == 0 && x < Q && rng() % 10 != 0) ? qs[x] : A[rng() % na]; }
     }
     int const dmax = static_cast<int>(std::max(ts[0].size(), ts[1].size()));
-    std::vector<U2> rowck(static_cast<size_t>((dmax + 31 + 3) / 4) * 128, U2{0xdeaddeadu, 0xdeaddeadu});
-    std::vector<U2> colck(static_cast<size_t>((dmax + 31 + CHUNK - 1) / CHUNK) * 32 * R, U2{0xdeaddeadu, 0xdeaddeadu});
+    std::vector<U2> rowck(row_elems(dmax), U2{0xdeaddeadu, 0xdeaddeadu});
+    std::vector<U2> colck(col_elems(dmax, R), U2{0xdeaddeadu, 0xdeaddeadu});
     std::vector<uint8_t> q4(Q);
     for (int i = 0; i < Q; i++) { q4[i] = oracle_map_4bit(static_cast<unsigned char>(qs[i])); }
     for (int h = 0; h < 2; h++) {

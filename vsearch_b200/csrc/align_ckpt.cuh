@@ -25,27 +25,13 @@
 #pragma once
 
 #include "align_kernels.cuh"
+#include "tb_ckpt.h"   // the checkpoint layout and the traceback that reads it
 
 namespace vsg {
 
-#ifndef VSG_CK_CHUNK
-#define VSG_CK_CHUNK 32
-#endif
-constexpr int CK_CHUNK = VSG_CK_CHUNK;   // steps per chunk = distance between column checkpoints (in steps): 16 or 32
-static_assert(CK_CHUNK == 16 || CK_CHUNK == 32, "chunk");
-#ifndef VSG_CK_SO_STEPS
-#define VSG_CK_SO_STEPS 8
-#endif
-constexpr int CK_SO_STEPS = VSG_CK_SO_STEPS;   // steps per trip of the score-only steady loop
-static_assert(CK_CHUNK % CK_SO_STEPS == 0, "score-only trip");
-
-// ---- checkpoint layout of one task (uint2 elements; .x/.y = the two values, low half = first target) ----
-// row checkpoints: element of (step s, lane l) — four consecutive steps of a lane share a 32-byte sector
-__host__ __device__ inline size_t ck_row_index(int s, int l) { return (static_cast<size_t>(s >> 2) * 32 + l) * 4 + (s & 3); }
-__host__ __device__ inline size_t ck_row_elems(int dmax) { return static_cast<size_t>((dmax + 31 + 3) >> 2) * 128; }
-// column checkpoints: state (H, E entering the next column) of lane l's row r after step 32k - 1, k >= 1
-__host__ __device__ inline size_t ck_col_index(int k, int l, int r, int R) { return (static_cast<size_t>(k - 1) * R + r) * 32 + l; }
-__host__ __device__ inline size_t ck_col_elems(int dmax, int R) { return static_cast<size_t>((dmax + 31 + CK_CHUNK - 1) / CK_CHUNK) * R * 32; }
+static_assert(ckpt::RMAX == FAST_RMAX, "tb_ckpt.h and align_kernels.cuh disagree");
+constexpr int CK_SO_STEPS = 8;   // steps per trip of the score-only steady loop
+static_assert(ckpt::CHUNK % CK_SO_STEPS == 0, "score-only trip");
 
 enum { CK_PROF = 0, CK_LUT = 1, CK_GEN = 2 };
 __host__ __device__ constexpr size_t ck_dyn_smem(int R, int mode)
@@ -241,16 +227,16 @@ nw_ckpt_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, DevSeqs ts,
     nxt_a = (cc < Dlo) ? (dlo_p[cc] & 15) : 0;
     nxt_b = (cc < Dhi) ? (dhi_p[cc] & 15) : 0;
   };
-  if (lane < CK_CHUNK && lane < dmax) { fetch(lane); }
+  if (lane < ckpt::CHUNK && lane < dmax) { fetch(lane); }
 
   int const cap_lo = Dlo - 1 + llast, cap_hi = Dhi - 1 + llast;
   uint32_t const geql2 = pk1(geql);
-  for (int s0 = 0; s0 < nsteps; s0 += CK_CHUNK) {
+  for (int s0 = 0; s0 < nsteps; s0 += ckpt::CHUNK) {
     {
       // publish columns [s0, s0+CHUNK): one column per lane; then start loading the next chunk's symbols
       __syncwarp();
       int const cc = s0 + lane;
-      if (lane < CK_CHUNK && cc < dmax) {
+      if (lane < ckpt::CHUNK && cc < dmax) {
         uint32_t x; uint2 yz;
         make_record(cc, nxt_a, nxt_b, x, yz);
         int const slot = cc & (RING - 1);
@@ -258,13 +244,13 @@ nw_ckpt_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, DevSeqs ts,
         rA[slot] = yz; rA[slot + RING] = yz;
       }
       __syncwarp();
-      if (lane < CK_CHUNK && cc + CK_CHUNK < dmax) { fetch(cc + CK_CHUNK); }
+      if (lane < ckpt::CHUNK && cc + ckpt::CHUNK < dmax) { fetch(cc + ckpt::CHUNK); }
     }
     uint32_t const slot0 = static_cast<uint32_t>(s0 - lane) & (RING - 1);
     // STEADY chunk: all 32 lanes inside the matrix, no score to pick up, and the target-gap penalties
     // uniform over the chunk's columns (neither target's last column is inside [s0-31, s0+31])
-    constexpr unsigned CH = CK_CHUNK;
-    bool const steady = (s0 >= 32) && (s0 + CK_CHUNK - 1 < dmax) &&
+    constexpr unsigned CH = ckpt::CHUNK;
+    bool const steady = (s0 >= 32) && (s0 + ckpt::CHUNK - 1 < dmax) &&
                         (static_cast<unsigned>(cap_lo - s0) >= CH) && (static_cast<unsigned>(cap_hi - s0) >= CH) &&
                         (static_cast<unsigned>(Dlo - 1 - (s0 - 31)) >= 31u + CH) && (static_cast<unsigned>(Dhi - 1 - (s0 - 31)) >= 31u + CH);
     if (steady) {
@@ -285,27 +271,27 @@ nw_ckpt_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, DevSeqs ts,
       };
       if (STORE) {
 #pragma unroll 1
-        for (int k0 = 0; k0 < CK_CHUNK; k0 += 4) {
+        for (int k0 = 0; k0 < ckpt::CHUNK; k0 += 4) {
           uint32_t ho[4], fo[4];
 #pragma unroll
           for (int u = 0; u < 4; u++) {
             step(aX + (k0 + u) * 4u);
             ho[u] = Hout; fo[u] = Fout;
           }
-          uint4 * const tp = reinterpret_cast<uint4 *>(myrow + ck_row_index(s0 + k0, lane));
+          uint4 * const tp = reinterpret_cast<uint4 *>(myrow + ckpt::row_index(s0 + k0, lane));
           tp[0] = make_uint4(ho[0], fo[0], ho[1], fo[1]);
           tp[1] = make_uint4(ho[2], fo[2], ho[3], fo[3]);
         }
       } else {
         // nothing to stage: eight steps per trip, the ring address the only per-trip arithmetic
 #pragma unroll 1
-        for (int k0 = 0; k0 < CK_CHUNK; k0 += CK_SO_STEPS, aX += CK_SO_STEPS * 4u) {
+        for (int k0 = 0; k0 < ckpt::CHUNK; k0 += CK_SO_STEPS, aX += CK_SO_STEPS * 4u) {
 #pragma unroll
           for (int u = 0; u < CK_SO_STEPS; u++) { step(aX + u * 4u); }
         }
       }
     } else {
-      int const kend = min(CK_CHUNK, nsteps - s0);
+      int const kend = min(ckpt::CHUNK, nsteps - s0);
       int c = s0 - lane;
       uint32_t aX = rX_s + slot0 * 4u, aA = rA_s + slot0 * 8u;
       for (int k = 0; k < kend; k++, c++, aX += 4u, aA += 8u) {
@@ -320,7 +306,7 @@ nw_ckpt_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, DevSeqs ts,
             fin = __vadd2(hin, yz.x);
           }
           column(x, yz.x, yz.y, hin, fin);
-          if (STORE) { myrow[ck_row_index(s0 + k, lane)] = make_uint2(Hout, Fout); }
+          if (STORE) { myrow[ckpt::row_index(s0 + k, lane)] = make_uint2(Hout, Fout); }
           if (capture && (c == Dlo - 1 || c == Dhi - 1)) {
             uint32_t v = 0;
 #pragma unroll
@@ -332,8 +318,8 @@ nw_ckpt_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, DevSeqs ts,
       }
     }
     // column checkpoint at the chunk's end (state after step s0 + 31); the last chunk needs none
-    if (STORE && s0 + CK_CHUNK < nsteps) {
-      uint2 * const cp = mycol + ck_col_index(s0 / CK_CHUNK + 1, lane, 0, R);
+    if (STORE && s0 + ckpt::CHUNK < nsteps) {
+      uint2 * const cp = mycol + ckpt::col_index(s0 / ckpt::CHUNK + 1, lane, 0, R);
 #pragma unroll
       for (int r = 0; r < R; r++) { cp[static_cast<size_t>(r) * 32] = make_uint2(Hl[r], E[r]); }
     }
@@ -345,17 +331,10 @@ nw_ckpt_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, DevSeqs ts,
   }
 }
 
-}  // namespace vsg
-
 // ---------------------------------------------------------------------------------------------
 // traceback over regenerated tiles (tb_ckpt.h): one thread per pair, the tile's direction bits in
 // shared memory (word-interleaved by thread: every thread owns one bank)
 // ---------------------------------------------------------------------------------------------
-#include "tb_ckpt.h"
-
-namespace vsg {
-
-static_assert(ckpt::CHUNK == CK_CHUNK && ckpt::RMAX == FAST_RMAX, "tb_ckpt.h and align_ckpt.cuh disagree");
 
 constexpr int TB_CK_THREADS = 128;
 
@@ -376,7 +355,7 @@ struct SmemBits {
 // steps are copied with cp.async — all in flight at once, no registers — into a thread-interleaved array
 // (vector v of thread t at [v][t]: every thread owns its own 16-byte bank group, so the divergent reads of a
 // warp's 32 unrelated walks never conflict).
-constexpr int TB_CK_ROWVECS = 2 * ((CK_CHUNK + 8) / 4);   // sectors of CHUNK + 2 steps at any alignment, x 2 x 16 bytes
+constexpr int TB_CK_ROWVECS = 2 * ((ckpt::CHUNK + 8) / 4);   // sectors of CHUNK + 2 steps at any alignment, x 2 x 16 bytes
 struct SmemRows {
   const uint2 * rowck;   // the task's row checkpoints
   uint4 * base;          // this thread's vector 0
@@ -386,7 +365,7 @@ struct SmemRows {
     int const g0 = s0 >> 2;
     int const g1 = s1 >> 2;
     sa = s0 & ~3;
-    const char * src = reinterpret_cast<const char *>(rowck + ck_row_index(s0 & ~3, l));
+    const char * src = reinterpret_cast<const char *>(rowck + ckpt::row_index(s0 & ~3, l));
     uint32_t dst = static_cast<uint32_t>(__cvta_generic_to_shared(base));
     for (int g = g0; g <= g1; g++) {
       asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" :: "r"(dst), "l"(src) : "memory");
@@ -407,7 +386,7 @@ struct SmemRows {
 
 constexpr size_t tb_ck_smem(int RT)
 {
-  return static_cast<size_t>(CK_CHUNK) * (RT / 8) * TB_CK_THREADS * 4 + static_cast<size_t>(TB_CK_ROWVECS) * TB_CK_THREADS * 16;
+  return static_cast<size_t>(ckpt::CHUNK) * (RT / 8) * TB_CK_THREADS * 4 + static_cast<size_t>(TB_CK_ROWVECS) * TB_CK_THREADS * 16;
 }
 
 template <int RT, bool TEXT>
@@ -441,11 +420,9 @@ __device__ __forceinline__ void traceback_ckpt_one(const ScoreParams & sp, const
   st[VSG_STAT_CIGARLEN] = TEXT ? cw.len : 0;
 }
 
-// statistics-only, straight from the forward tasks: pair 2k / 2k+1 = first / second target of task k.
-// Alignments differ a lot in the number of tiles their paths cross (the end gap of a short query in a long target
-// alone is up to D/32 tiles), so a thread does not own one pair: the grid is sized to fill the device once, every
-// thread starts with pair = its global index and, whenever its alignment is finished, takes the next unclaimed pair
-// from a ticket counter while the other lanes of its warp carry on with theirs.  *ticket must be 0 at launch.
+// statistics-only, straight from the forward tasks: pair 2k / 2k+1 = first / second target of task k.  One thread
+// per pair: thread i walks pair i (gate.ids[i] when the launch is gated), and the lanes of a warp run their walks'
+// rounds together until the last of them is done.
 // TRACEBACK ON DEMAND (the batched search driver).  align_delayed hands search16 a group of up to eight candidates of
 // a query and then examines them in order until the accept / reject limits are reached (searchcore.cpp:780-880): when
 // the first one is accepted and that accept is the last one wanted, the other seven alignments are never looked at.
@@ -491,31 +468,28 @@ template <int RT, bool GENERAL>
 __device__ __forceinline__ void traceback_ckpt_tasks_body(const ScoreParams & sp, const DevSeqs & qs, const DevSeqs & ts,
                                                           const FastTask * __restrict__ tasks, int ntasks, int R,
                                                           const uint2 * __restrict__ rowck, const uint2 * __restrict__ colck,
-                                                          int32_t * __restrict__ stats, int * __restrict__ ticket, int ticket_base,
-                                                          const TbGate & gate, unsigned char * smem)
+                                                          int32_t * __restrict__ stats, const TbGate & gate, unsigned char * smem)
 {
   int const total = gate.ids != nullptr ? gate.nids : 2 * ntasks;
-  int const nthreads = gridDim.x * blockDim.x;
+  int const p = blockIdx.x * blockDim.x + threadIdx.x;
   SmemRows rows{nullptr, reinterpret_cast<uint4 *>(smem) + threadIdx.x};
   SmemBits<RT / 8> bits{reinterpret_cast<uint32_t *>(smem + static_cast<size_t>(TB_CK_ROWVECS) * TB_CK_THREADS * 16) + threadIdx.x};
   auto emit = [](char, int) {};
   ckpt::Walk<RT, GENERAL> w;
-  int next = blockIdx.x * blockDim.x + threadIdx.x;
   int out = -1;
   int myQ = 0, myD = 0;
   bool active = false;
-  for (;;) {
-    while (!active && next < total) {
-      int const id = gate.ids != nullptr ? gate.ids[next] : next;
-      FastTask const tk = tasks[id >> 1];
-      int const half = id & 1;
-      out = half ? tk.out_hi : tk.out_lo;
-      next = ticket_base >= total ? total : nthreads + atomicAdd(ticket, 1);
-      if (out < 0) { continue; }
-      if (gate.leader_of != nullptr && gate.phase == 2) {
-        int const lead = gate.leader_of[out];
-        if (lead >= 0 && stats[static_cast<size_t>(lead) * VSG_STAT_WORDS + VSG_STAT_CIGARLEN] == TB_VERDICT_ACCEPTED) { continue; }
-      }
+  if (p < total) {
+    int const id = gate.ids != nullptr ? gate.ids[p] : p;
+    FastTask const tk = tasks[id >> 1];
+    int const half = id & 1;
+    out = half ? tk.out_hi : tk.out_lo;
+    active = out >= 0;
+    if (active && gate.leader_of != nullptr && gate.phase == 2) {
+      int const lead = gate.leader_of[out];
+      active = !(lead >= 0 && stats[static_cast<size_t>(lead) * VSG_STAT_WORDS + VSG_STAT_CIGARLEN] == TB_VERDICT_ACCEPTED);
+    }
+    if (active) {
       uint32_t const q = tk.q, t = half ? tk.thi : tk.tlo;
       ckpt::PairView pv;
       pv.rowck = reinterpret_cast<const ckpt::U2 *>(rowck + tk.dir_off);
@@ -526,9 +500,9 @@ __device__ __forceinline__ void traceback_ckpt_tasks_body(const ScoreParams & sp
       myQ = pv.Q; myD = pv.D;
       rows.rowck = rowck + tk.dir_off;
       w.start(pv);
-      active = true;
     }
-    if (!__any_sync(0xffffffffu, active)) { break; }
+  }
+  while (__any_sync(0xffffffffu, active)) {
     if (active) {
       if (w.running()) { w.round(sp, bits, rows, emit); }
       if (!w.running()) {
@@ -550,11 +524,11 @@ __global__ void __launch_bounds__(TB_CK_THREADS)
 traceback_ckpt_tasks_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, DevSeqs ts,
                             const FastTask * __restrict__ tasks, int ntasks, int R, int general,
                             const uint2 * __restrict__ rowck, const uint2 * __restrict__ colck,
-                            int32_t * __restrict__ stats, int * __restrict__ ticket, int ticket_base, TbGate gate)
+                            int32_t * __restrict__ stats, TbGate gate)
 {
   extern __shared__ __align__(16) unsigned char tb_smem[];
-  if (general) { traceback_ckpt_tasks_body<RT, true>(sp, qs, ts, tasks, ntasks, R, rowck, colck, stats, ticket, ticket_base, gate, tb_smem); }
-  else { traceback_ckpt_tasks_body<RT, false>(sp, qs, ts, tasks, ntasks, R, rowck, colck, stats, ticket, ticket_base, gate, tb_smem); }
+  if (general) { traceback_ckpt_tasks_body<RT, true>(sp, qs, ts, tasks, ntasks, R, rowck, colck, stats, gate, tb_smem); }
+  else { traceback_ckpt_tasks_body<RT, false>(sp, qs, ts, tasks, ntasks, R, rowck, colck, stats, gate, tb_smem); }
 }
 
 // with CIGAR text, from pair descriptors (kind 2 = checkpoint layout; the others belong to traceback_kernel)

@@ -33,19 +33,9 @@ namespace vsg {
 constexpr int SHARD_BITS = 15;
 constexpr int SHARD = 1 << SHARD_BITS;  // targets per shard
 constexpr int RANK_THREADS = 512;
-#ifndef VSG_RANK_U
-#define VSG_RANK_U 4      // posting vectors (of 8) a lane holds at a time
-#endif
-#ifndef VSG_RANK_ROLL
-#define VSG_RANK_ROLL 0   // 1: refill a slot as soon as it has been applied (measured: no gain, see DESIGN experiment log)
-#endif
-#ifndef VSG_RANK_ZFUSE
-#define VSG_RANK_ZFUSE 1  // clear the counters behind the last scan of a shard instead of in a pass of its own
-#endif
 constexpr int KMER_CAP = 2048;          // distinct-k-mer capacity per query (query length <= 2047 + k)
 constexpr int CAND_CAP = 2048;          // candidate keys held in shared memory
 constexpr int TOPHITS_MAX = 1024;
-constexpr int RANK_PREFETCH = 3;         // k-mers (per warp) between the L2 prefetch of a list and its use
 constexpr int SCAN_SEG_WORDS = 512;     // counters are scanned 1024 at a time (<= 1024 new candidates)
 constexpr int COUNTER_WORDS = SHARD / 2 + 1;
 // Static index: a shard holds 32766 targets and its postings are stored as the BYTE OFFSET of the target's counter
@@ -282,7 +272,7 @@ __global__ void __launch_bounds__(RANK_THREADS, 2)
 rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restrict__ shards, int nshards,
             int k, int mask_lower, int minwordmatches, int tophits,
             uint32_t * __restrict__ out_seqno, uint32_t * __restrict__ out_count, int32_t * __restrict__ out_n,
-            int32_t * __restrict__ status, uint32_t * __restrict__ scratch, size_t scratch_stride, int bitmap_words, int flat)
+            int32_t * __restrict__ status, uint32_t * __restrict__ scratch, size_t scratch_stride, int bitmap_words)
 {
   extern __shared__ __align__(16) unsigned char smem[];
   uint64_t * const cand = reinterpret_cast<uint64_t *>(smem);                     // CAND_CAP
@@ -455,10 +445,7 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
       __syncthreads();
       // 3. postings -> counters (targets within a list are distinct, lists collide -> shared-memory
       //    atomics).  Lists are 16-byte aligned and padded, so a lane pulls 8 targets per 128-bit
-      //    load.  A warp walks the two sub-lists of a k-mer at a time and issues up to three loads per lane and
-      //    sub-list before it touches a counter: six independent HBM requests per lane hide the latency that a
-      //    one-list-at-a-time loop exposes once per list.  Padding entries land in counter word 16383, which
-      //    no target of a static shard owns.
+      //    load.  Padding entries land in counter word 16383, which no target of a static shard owns.
       if constexpr (INCR) {
         // unpadded lists of 32-bit target numbers: one warp per list, coalesced loads
         for (int li = warp; li < np2; li += NWARPS) {
@@ -469,12 +456,7 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
             atomicAdd(&counters[a >> 1], (a & 1) ? 0x10000u : 1u);
           }
         }
-      }
-#ifdef VSG_RANK_LEGACY
-      else if (flat != 0) {
-#else
-      else {
-#endif
+      } else {
         // FLAT VECTOR STREAM.  The even and the odd sub-list of a k-mer are one contiguous run of 16-byte vectors, and
         // the runs of all the query's k-mers, laid end to end, form one virtual stream of Vtot vectors.  Each warp
         // takes a contiguous 1/16 of the stream and walks it 32 vectors per round — every lane always has a vector
@@ -524,7 +506,7 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
         uint32_t const wbeg = static_cast<uint32_t>(warp) * per_w;
         uint32_t const wend = min(Vtot, wbeg + per_w);
         if (wbeg < wend) {
-          constexpr int U = VSG_RANK_U;   // vectors (of 8 postings) held per lane
+          constexpr int U = 4;   // vectors (of 8 postings) held per lane
           const uint4 * __restrict__ pbase = reinterpret_cast<const uint4 *>(S.post);
           uint32_t const cnt_sa = static_cast<uint32_t>(__cvta_generic_to_shared(counters));
           // the run holding this lane's first vector: the first whose end lies beyond it
@@ -538,7 +520,7 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
           uint32_t sa = static_cast<uint32_t>(__cvta_generic_to_shared(lbeg + lo));
           uint32_t ce = cum[lo];
           // U loads per lane are issued back to back, then turned into counter updates; the other 31 warps of the SM
-          // cover the wait (VSG_RANK_ROLL refills each slot right after its use instead: measured equal).
+          // cover the wait
           uint4 cur[U];
           uint32_t inc[U];
           auto fetch = [&](int u, uint32_t vv) {
@@ -566,100 +548,14 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
               }
             }
           };
-#if VSG_RANK_ROLL
-#pragma unroll
-          for (int u = 0; u < U; u++) { fetch(u, wbeg + 32u * u + static_cast<uint32_t>(lane)); }
-          for (uint32_t v0 = wbeg; v0 < wend; v0 += 32u * U) {
-#pragma unroll
-            for (int u = 0; u < U; u++) {
-              apply(u);
-              fetch(u, v0 + 32u * (U + u) + static_cast<uint32_t>(lane));
-            }
-          }
-#else
           for (uint32_t v0 = wbeg; v0 < wend; v0 += 32u * U) {
 #pragma unroll
             for (int u = 0; u < U; u++) { fetch(u, v0 + 32u * u + static_cast<uint32_t>(lane)); }
 #pragma unroll
             for (int u = 0; u < U; u++) { apply(u); }
           }
-#endif
-        }
-#ifdef VSG_RANK_LEGACY
-      } else {
-        // (A/B reference, VSG_RANK_FLAT=0) a warp takes one k-mer at a time: list a = its even targets (increment 1),
-        // list b = its odd targets (increment 0x10000)
-        auto pair_len = [&](int li) -> uint32_t {
-          uint32_t const na = llen[li] & 0xffffu, nb = llen[li] >> 16;
-          return na > nb ? na : nb;
-        };
-        // One register buffer of six vectors (three per list): as soon as a vector has been turned into
-        // counter updates its slot is refilled from the NEXT (k-mer, offset), so six loads per lane
-        // stay in flight without a second buffer (48 data registers would not leave room in the 64
-        // this kernel may use at two 512-thread CTAs per SM).
-        struct ListPair { uint32_t na, nb; const uint4 * pa; const uint4 * pb; };
-        auto bounds_of = [&](int li) -> ListPair {
-          ListPair lp;
-          lp.na = llen[li] & 0xffffu;
-          lp.nb = llen[li] >> 16;
-          lp.pa = reinterpret_cast<const uint4 *>(S.post + lbeg[li]);
-          lp.pb = lp.pa + lp.na;
-          return lp;
-        };
-        int li = warp;
-        uint32_t base = 0;
-        bool have = li < np2;
-        uint4 cur[6];
-        uint32_t valid = 0;
-        if (have) {
-          ListPair const lp = bounds_of(li);
-#pragma unroll
-          for (int u = 0; u < 6; u++) {
-            uint32_t const e = lane + 32u * (u % 3);
-            if (e < (u < 3 ? lp.na : lp.nb)) { cur[u] = __ldg((u < 3 ? lp.pa : lp.pb) + e); valid |= 1u << u; }
-          }
-        }
-        while (have) {
-          int nli = li;
-          uint32_t nbase = base + 96;
-          if (nbase >= pair_len(li)) { nli = li + NWARPS; nbase = 0; }
-          bool const nhave = nli < np2;
-          if (nbase == 0) {
-            // the register buffer only reaches one k-mer ahead, less than a trip to HBM takes: pull the k-mer three
-            // turns ahead into L2 now (its two sub-lists are one contiguous run of 128-byte lines, one line per lane)
-            int const pli = nli + RANK_PREFETCH * NWARPS;
-            if (pli < np2) {
-              uint32_t const pn = (llen[pli] & 0xffffu) + (llen[pli] >> 16);   // vectors of 16 bytes
-              if (8u * lane < pn) {
-                asm volatile("prefetch.global.L2 [%0];" :: "l"(S.post + lbeg[pli] + 64u * lane));
-              }
-            }
-          }
-          ListPair lp{0u, 0u, nullptr, nullptr};
-          if (nhave) { lp = bounds_of(nli); }
-          uint32_t nvalid = 0;
-#pragma unroll
-          for (int u = 0; u < 6; u++) {
-            if ((valid & (1u << u)) != 0u) {
-              uint32_t const w[4] = {cur[u].x, cur[u].y, cur[u].z, cur[u].w};
-              uint32_t const inc = u < 3 ? 1u : 0x10000u;
-#pragma unroll
-              for (int k = 0; k < 4; k++) {
-                uint32_t const a = w[k] & 0xffffu, b = w[k] >> 16;   // byte offsets of the counter words
-                atomicAdd(reinterpret_cast<uint32_t *>(reinterpret_cast<unsigned char *>(counters) + a), inc);
-                atomicAdd(reinterpret_cast<uint32_t *>(reinterpret_cast<unsigned char *>(counters) + b), inc);
-              }
-            }
-            uint32_t const e = nbase + lane + 32u * (u % 3);
-            if (e < (u < 3 ? lp.na : lp.nb)) { cur[u] = __ldg((u < 3 ? lp.pa : lp.pb) + e); nvalid |= 1u << u; }
-          }
-          valid = nvalid;
-          li = nli; base = nbase; have = nhave;
         }
       }
-#else
-      }
-#endif
       __syncthreads();
       }  // chunk
       int const nwords = (S.nt + 1) >> 1;
@@ -695,11 +591,11 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
         int const K = s_K;
         if (level + K <= CAND_CAP) {
           // at most K targets (all shards so far) are >= T1, so at most K keys are appended here
-          scan_counters(S.nt, T1, VSG_RANK_ZFUSE, [&](uint32_t c, int lt) {
+          scan_counters(S.nt, T1, 1, [&](uint32_t c, int lt) {
             int const t = S.t0 + lt;
             cand[atomicAdd(&s_ncand, 1)] = make_key(c, static_cast<uint32_t>(db.len[t]), static_cast<uint32_t>(t));
           });
-          clean = VSG_RANK_ZFUSE != 0;
+          clean = true;
           __syncthreads();
           continue;  // next shard
         }
@@ -863,8 +759,7 @@ namespace vsg {
 
 static void shard_bank_order(vsg_ctx * c, const uint32_t * start, uint16_t * post, size_t nlists)
 {
-  static bool const bank_order = [] { const char * e = std::getenv("VSG_BANK_ORDER"); return e == nullptr || e[0] != '0'; }();
-  if (!bank_order || nlists == 0) { return; }
+  if (nlists == 0) { return; }
   int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
   list_bank_order_kernel<<<static_cast<int>(std::min<size_t>(nlists, static_cast<size_t>(sms) * 32)), 128, 0, c->stream>>>(start, post, static_cast<int>(nlists));
@@ -1145,12 +1040,11 @@ int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, 
     if ((rc = c->rank_scratch.reserve(sizeof(uint32_t) * stride * static_cast<size_t>(grid))) != VSG_OK) { return rc; }
     d_scratch = static_cast<uint32_t *>(c->rank_scratch.p);
   }
-  static int const rank_flat = [] { const char * e = std::getenv("VSG_RANK_FLAT"); return (e == nullptr || e[0] != '0') ? 1 : 0; }();
   VSG_CUDA_OK(cudaEventRecord(c->ev[4], rs));
   rank_kernel<false><<<grid, RANK_THREADS, RANK_SMEM, rs>>>(
       queries->d, q0, static_cast<int>(nq), ix->db->d, static_cast<const ShardDev *>(ix->b_shards.p),
       static_cast<int>(ix->h_shards.size()), ix->k, mask_lower, minwordmatches, tophits, *d_seqno, *d_count, *d_n,
-      *d_status, d_scratch, stride, bitmap_words, rank_flat);
+      *d_status, d_scratch, stride, bitmap_words);
   count_launch();
   VSG_CUDA_OK(cudaEventRecord(c->ev[5], rs));
   c->rank_pending = true;
@@ -1390,7 +1284,7 @@ int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, in
   }
   rank_kernel<true><<<grid, RANK_THREADS, RANK_SMEM, c->stream>>>(
       queries->d, q0, static_cast<int>(nq), lens, static_cast<const ShardDev *>(ix->b_shards.p), nshards, ix->k, ix->mask_lower,
-      minwordmatches, tophits, *d_seqno, *d_count, *d_n, *d_status, d_scratch, stride, bitmap_words, 0);
+      minwordmatches, tophits, *d_seqno, *d_count, *d_n, *d_status, d_scratch, stride, bitmap_words);
   count_launch();
   return VSG_OK;
 }

@@ -184,8 +184,6 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
   int nthreads = 8;
   if (const char * e = std::getenv("VSG_HOST_THREADS")) { nthreads = std::max(1, std::atoi(e)); }
   nthreads = static_cast<int>(std::min<int64_t>(nthreads, nbatches));
-  bool stagger = true;
-  if (const char * e = std::getenv("VSG_STAGGER")) { stagger = std::atoi(e) != 0; }
   int64_t tail_pairs = 4096;  // the tail starts when the round's pairs + all remaining candidates fit in this (0: never)
   if (const char * e = std::getenv("VSG_TAIL_PAIRS")) { tail_pairs = std::max<int64_t>(0, std::atoll(e)); }
   while (static_cast<int>(c->children.size()) < nthreads) {
@@ -652,7 +650,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
     bool first = true;
     for (;;) {
       int64_t want = BATCH;
-      if (first && stagger && nthreads > 1) { want = std::max<int64_t>(256, BATCH * (t + 1) / nthreads); }
+      if (first && nthreads > 1) { want = std::max<int64_t>(256, BATCH * (t + 1) / nthreads); }
       first = false;
       int64_t const b0 = next.fetch_add(want);
       if (b0 >= nq) { break; }

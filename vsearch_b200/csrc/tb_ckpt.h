@@ -33,17 +33,20 @@
 namespace vsg {
 namespace ckpt {
 
-#ifndef VSG_CK_CHUNK
-#define VSG_CK_CHUNK 32
-#endif
-constexpr int CHUNK = VSG_CK_CHUNK;   // CK_CHUNK of align_ckpt.cuh
+constexpr int CHUNK = 32;   // steps per chunk = distance between column checkpoints (in steps)
 constexpr int RMAX = 16;    // rows per lane
 
 struct U2 { uint32_t x, y; };  // layout of CUDA's uint2
 
-// the layout functions of align_ckpt.cuh, restated for host compilation (static_asserted equal there)
+// ---- checkpoint layout of one task (U2 / uint2 elements; .x/.y = the two values, low half = first target) ----
+// The forward kernel writes it, the traceback reads it, and the host model of tools/ckpt_host_check.cpp writes it
+// for the host traceback: all three use these functions.
+// row checkpoints: element of (step s, lane l) — four consecutive steps of a lane share a 32-byte sector
 VSG_CKPT_HD size_t row_index(int s, int l) { return (static_cast<size_t>(s >> 2) * 32 + l) * 4 + (s & 3); }
+VSG_CKPT_HD size_t row_elems(int dmax) { return static_cast<size_t>((dmax + 31 + 3) >> 2) * 128; }
+// column checkpoints: state (H, E entering the next column) of lane l's row r after step 32k - 1, k >= 1
 VSG_CKPT_HD size_t col_index(int k, int l, int r, int R) { return (static_cast<size_t>(k - 1) * R + r) * 32 + l; }
+VSG_CKPT_HD size_t col_elems(int dmax, int R) { return static_cast<size_t>((dmax + 31 + CHUNK - 1) / CHUNK) * R * 32; }
 
 struct PairView {
   const U2 * rowck;   // the task's row checkpoints
@@ -190,8 +193,8 @@ inline void HostBits::stage_word(int bj, const uint8_t * t, int D, int mis, int 
 // half is real, or both) can only borrow out of bit 31.
 // GENERAL: a symbol outside ACGT in either sequence (scores from the 16x16 table instead of match / mismatch).
 // One alignment's traceback as a resumable object: start(), then round() once per tile while running(), then
-// finish().  The kernels keep one of these per thread; a thread whose alignment is finished can start the next one
-// while its warp's other lanes are still in the middle of theirs (align_ckpt.cuh).
+// finish().  The statistics-only kernel keeps one of these per thread and runs the rounds of a warp's 32 walks
+// together (align_ckpt.cuh).
 template <int RT, bool GENERAL>
 struct Walk {
   PairView v;

@@ -236,7 +236,6 @@ extern "C" int vsg_ctx_create(int device, const vsg_scoring * scoring, vsg_ctx *
   build_score_params(*scoring, c->sp);
   c->sp.shift = 0;
   c->ckpt_enabled = shifted_params(c->sp, c->sp2);
-  if (const char * ck = std::getenv("VSG_CKPT")) { if (ck[0] == '0') { c->ckpt_enabled = false; } }
   const char * df = std::getenv("VSG_DISABLE_FAST");
   c->fast_disabled = (df != nullptr && df[0] == '1');
   const char * db = std::getenv("VSG_DIR_BUDGET_MB");
@@ -276,7 +275,7 @@ extern "C" void vsg_ctx_destroy(vsg_ctx * c)
   if (c->stream != nullptr) { cudaStreamSynchronize(c->stream); }
   for (DevBuf * b : {&c->dir, &c->bnd, &c->he, &c->cigar_scratch, &c->cigar_dense, &c->stats,
                      &c->tasks_fast, &c->tasks_exact, &c->pairs, &c->cigar_len, &c->cigar_offs,
-                     &c->cub_tmp, &c->rank_tmp, &c->rank_scratch, &c->pre_flags, &c->ticket, &c->rerun_count}) { b->release(); }
+                     &c->cub_tmp, &c->rank_tmp, &c->rank_scratch, &c->pre_flags, &c->gate, &c->rerun_count}) { b->release(); }
   for (PinBuf * b : {&c->h_tasks, &c->h_stats}) { b->release(); }
   for (auto & ev : c->ev) { if (ev != nullptr) { cudaEventDestroy(ev); } }
   for (auto & ev : c->ev_pool) { cudaEventDestroy(ev); }
@@ -511,8 +510,6 @@ void launch_ckpt(vsg_ctx * c, int R, bool general, int write, const DevSeqs & qs
     }
     return;
   }
-  static const bool force_lut = std::getenv("VSG_CK_LUT") != nullptr;   // experiment: table variant (more resident warps) for R <= 8 too
-  if (force_lut && R == 8) { launch_ckpt_write<8, CK_LUT>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); return; }
   switch (R) {
 #define VSG_CASE(r) case r: launch_ckpt_write<r, CK_PROF>(c, write, qs, ts, d_tasks, n, leader_of, rerun_count); break;
     VSG_CASE(1) VSG_CASE(2) VSG_CASE(3) VSG_CASE(4) VSG_CASE(5) VSG_CASE(6) VSG_CASE(7) VSG_CASE(8)
@@ -524,39 +521,25 @@ void launch_ckpt(vsg_ctx * c, int R, bool general, int write, const DevSeqs & qs
   }
 }
 
-int launch_tb_ckpt_tasks(vsg_ctx * c, int R, bool general, const DevSeqs & qs, const DevSeqs & ts, const FastTask * d_tasks, int n,
-                         const TbGate & gate)
+template <int RT>
+void launch_tb_ckpt_tasks_rt(vsg_ctx * c, int nthr, int R, bool general, const DevSeqs & qs, const DevSeqs & ts,
+                             const FastTask * d_tasks, int n, const TbGate & gate)
 {
-  // a grid that fills the device once (the kernel hands further pairs out itself), fewer blocks for small calls
-  int rc;
-  if ((rc = c->ticket.reserve(64)) != VSG_OK) { return rc; }
-  VSG_CUDA_OK(cudaMemsetAsync(c->ticket.p, 0, sizeof(int), c->stream));
-  int sms = 132;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
-  int const nthr = gate.ids != nullptr ? gate.nids : 2 * n;
-  if (nthr == 0) { return VSG_OK; }
-  int const want = (nthr + TB_CK_THREADS - 1) / TB_CK_THREADS;
-  static int const refill = [] { const char * e = std::getenv("VSG_TB_REFILL"); return e != nullptr ? std::atoi(e) : 0; }();
-  int const tbase = refill > 0 ? 0 : nthr;   // >= the number of pairs: every thread does its own pair only
-  if (R <= 8) {
-    cudaFuncSetAttribute(traceback_ckpt_tasks_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tb_ck_smem(8)));
-    int per_sm = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, traceback_ckpt_tasks_kernel<8>, TB_CK_THREADS, tb_ck_smem(8));
-    int const blocks = refill > 0 ? std::min(want, std::max(1, per_sm) * sms * refill) : want;
-    traceback_ckpt_tasks_kernel<8><<<blocks, TB_CK_THREADS, tb_ck_smem(8), c->stream>>>(
-        c->sp2, qs, ts, d_tasks, n, R, general ? 1 : 0, static_cast<const uint2 *>(c->dir.p), static_cast<const uint2 *>(c->bnd.p),
-        static_cast<int32_t *>(c->stats.p), static_cast<int *>(c->ticket.p), tbase, gate);
-  } else {
-    cudaFuncSetAttribute(traceback_ckpt_tasks_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tb_ck_smem(16)));
-    int per_sm = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, traceback_ckpt_tasks_kernel<16>, TB_CK_THREADS, tb_ck_smem(16));
-    int const blocks = refill > 0 ? std::min(want, std::max(1, per_sm) * sms * refill) : want;
-    traceback_ckpt_tasks_kernel<16><<<blocks, TB_CK_THREADS, tb_ck_smem(16), c->stream>>>(
-        c->sp2, qs, ts, d_tasks, n, R, general ? 1 : 0, static_cast<const uint2 *>(c->dir.p), static_cast<const uint2 *>(c->bnd.p),
-        static_cast<int32_t *>(c->stats.p), static_cast<int *>(c->ticket.p), tbase, gate);
-  }
+  cudaFuncSetAttribute(traceback_ckpt_tasks_kernel<RT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tb_ck_smem(RT)));
+  traceback_ckpt_tasks_kernel<RT><<<(nthr + TB_CK_THREADS - 1) / TB_CK_THREADS, TB_CK_THREADS, tb_ck_smem(RT), c->stream>>>(
+      c->sp2, qs, ts, d_tasks, n, R, general ? 1 : 0, static_cast<const uint2 *>(c->dir.p), static_cast<const uint2 *>(c->bnd.p),
+      static_cast<int32_t *>(c->stats.p), gate);
   count_launch();
-  return VSG_OK;
+}
+
+// statistics-only traceback of checkpoint tasks, one thread per pair (align_ckpt.cuh)
+void launch_tb_ckpt_tasks(vsg_ctx * c, int R, bool general, const DevSeqs & qs, const DevSeqs & ts, const FastTask * d_tasks, int n,
+                          const TbGate & gate)
+{
+  int const nthr = gate.ids != nullptr ? gate.nids : 2 * n;
+  if (nthr == 0) { return; }
+  if (R <= 8) { launch_tb_ckpt_tasks_rt<8>(c, nthr, R, general, qs, ts, d_tasks, n, gate); }
+  else { launch_tb_ckpt_tasks_rt<16>(c, nthr, R, general, qs, ts, d_tasks, n, gate); }
 }
 
 // A chunk = the tasks whose direction blocks share the scratch buffer at the same time.
@@ -788,8 +771,8 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
         // single-strip tasks go through the checkpoint kernel (no direction bits; align_ckpt.cuh) when its
         // shifted scoring stays inside the exact range too
         bool const ck = (ns == 1) && c->ckpt_enabled && (ckpt_any_size || dmax >= 3 * Q) && fast_path_ok(fbound2, 32 * R, dmax);
-        uint64_t const dirb = ck ? ck_row_elems(dmax) * sizeof(uint2) : static_cast<uint64_t>(ns) * fast_strip_bytes(dmax, R);
-        uint64_t const auxe = ck ? ck_col_elems(dmax, R) : (ns > 1 ? static_cast<uint64_t>(dmax) : 0);
+        uint64_t const dirb = ck ? ckpt::row_elems(dmax) * sizeof(uint2) : static_cast<uint64_t>(ns) * fast_strip_bytes(dmax, R);
+        uint64_t const auxe = ck ? ckpt::col_elems(dmax, R) : (ns > 1 ? static_cast<uint64_t>(dmax) : 0);
         if (!cb.empty() && cb.dir_bytes + dirb + (cb.bnd_elems + auxe) * sizeof(uint2) > c->dir_budget) { close_chunk(); }
         FastTask ft{};
         ft.q = q; ft.tlo = a.t; ft.thi = b.t;
@@ -927,7 +910,7 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
           if (!run.ckpt) { continue; }
           GateRun const & g = gate_runs[ci][ri];
           TbGate const g1{d_gate_ids + g.lead_first, static_cast<int>(g.lead_count), d_leader, 1, gate_iddef, gate_threshold};
-          if ((rc = launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, g1)) != VSG_OK) { return rc; }
+          launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, g1);
         }
         // the checkpoints of the score-only tasks phase 2 will walk (a follower whose leader was not accepted)
         for (auto const & run : pl.runs) {
@@ -942,10 +925,10 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
           if (gated) {
             GateRun const & g = gate_runs[ci][ri];
             TbGate const g2{d_gate_ids + g.foll_first, static_cast<int>(g.foll_count), d_leader, 2, gate_iddef, gate_threshold};
-            if ((rc = launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, g2)) != VSG_OK) { return rc; }
+            launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, g2);
             continue;
           }
-          if ((rc = launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, no_gate)) != VSG_OK) { return rc; }
+          launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, no_gate);
           continue;
         }
         int const nthr = 2 * run.count;

@@ -128,11 +128,11 @@ struct vsg_ctx {
   vsg_scoring scoring{};
   vsg::ScoreParams sp{};
   vsg::ScoreParams sp2{};      // the shifted scoring the checkpoint kernels run with (align_ckpt.cuh)
-  bool ckpt_enabled = true;    // VSG_CKPT=0 routes single-strip pairs through the direction-bit kernel instead (A/B, tests)
+  bool ckpt_enabled = true;    // false when the shifted scoring does not fit (shifted_params): direction-bit kernels only
   bool fast_disabled = false;  // VSG_DISABLE_FAST=1 (tests force the exact kernel)
   // scratch
   vsg::DevBuf dir, bnd, he, cigar_scratch, cigar_dense, stats, tasks_fast, tasks_exact, pairs,
-      cigar_len, cigar_offs, cub_tmp, rank_tmp, rank_scratch, pre_flags, ticket, gate, rerun_count;
+      cigar_len, cigar_offs, cub_tmp, rank_tmp, rank_scratch, pre_flags, gate, rerun_count;
   vsg::PinBuf h_tasks, h_stats;
   size_t dir_budget = (size_t)64 << 30;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
