@@ -319,6 +319,52 @@ def test_deferred_pairs_go_through_the_fallback_callback(ctx):
     ix.close(); db.close(); qs.close()
 
 
+@pytest.mark.parametrize("driver", ["allpairs", "cluster_fast"])
+def test_allpairs_and_cluster_defer_pairs_to_the_fallback_callback(ctx, driver):
+    """all-pairs and cluster_fast resolve deferred pairs through vsg_ctx_set_fallback too: with a gap penalty that does
+    not fit a 16-bit cell every pair is deferred, and a callback answering with the default scoring's alignments gives
+    the default context's rows field for field"""
+    reads = synth.config1_allpairs(n_reads=72, n_roots=4, length=200, seed=47)
+    n = len(reads)
+    qi, ti = (x.ravel() for x in np.meshgrid(np.arange(n), np.arange(n), indexing="ij"))
+    ss = ctx.seqset(reads)
+    al = ctx.align_pairs(ss, ss, qi, ti)
+    ss.close()
+    table = {(int(qi[k]), int(ti[k])): [int(al.score[k]), int(al.aligned[k]), int(al.matches[k]), int(al.mismatches[k]),
+                                        int(al.gaps[k])] + [int(v) for v in al.trims[k]] for k in range(qi.shape[0])}
+    o = vlib.default_search_opts(); o.id = 0.8
+
+    def run(c):
+        s = c.seqset(reads)
+        try:
+            if driver == "allpairs":
+                return vlib.allpairs(c, s, 0, n, o, n * n)[0].tolist()
+            res, ncl, _ = vlib.cluster_fast(c, s, o, 8)
+            return res.tolist(), ncl
+        finally:
+            s.close()
+
+    want = run(ctx)
+    pen = np.array(vlib.DEFAULT_PEN, dtype=np.int64); pen[4] = 2 ** 31 - 1   # does not fit a cell: everything deferred
+    c2 = vlib.Context(0, pen=pen)
+    try:
+        with pytest.raises(vlib.VsgError, match="linear-memory aligner"):
+            run(c2)
+
+        def fallback(q, strand, t):
+            assert strand == 0
+            return table[(q, t)]
+        c2.set_fallback(fallback)
+        got = run(c2)
+    finally:
+        c2.close()
+    if driver == "allpairs":
+        assert len(want) > 0
+    else:
+        assert want[1] < n   # some reads joined a cluster
+    assert got == want
+
+
 def test_long_queries_rank_vs_oracle(ctx):
     """queries with more than 2048 k-mer windows take the HBM de-duplication path of the ranker"""
     rng = np.random.default_rng(43)

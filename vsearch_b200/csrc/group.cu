@@ -5,11 +5,11 @@
 // (shim/search_batch_vsg.cpp with VSG_DEVICES=0,1,...).  bench.py's multi-GPU runs keep one process per
 // GPU with an NCCL broadcast, as its contract asks; both end in the same per-device calls.
 #include "vsg_internal.h"
+#include "workers.h"
 
 #include <algorithm>
 #include <chrono>
 #include <cstring>
-#include <thread>
 
 using namespace vsg;
 
@@ -116,21 +116,12 @@ extern "C" int vsg_group_create(const int * devices, int ndev, const vsg_scoring
   g->broadcast_ms = now_ms() - t0;
   // 3. every device builds its own index (a few ms; cheaper than shipping 2 B per posting)
   t0 = now_ms();
-  std::vector<int> rcs(static_cast<size_t>(ndev), VSG_OK);
-  std::vector<std::string> msgs(static_cast<size_t>(ndev));
-  std::vector<std::thread> pool;
-  for (int i = 0; i < ndev; i++) {
-    pool.emplace_back([&, i]() {
-      rcs[static_cast<size_t>(i)] = vsg_index_create(g->ctx[static_cast<size_t>(i)], g->db[static_cast<size_t>(i)], wordlength, g->mask_lower,
-                                                     &g->index[static_cast<size_t>(i)]);
-      if (rcs[static_cast<size_t>(i)] != VSG_OK) { msgs[static_cast<size_t>(i)] = vsg_last_error(); }
-    });
-  }
-  for (auto & th : pool) { th.join(); }
+  rc = run_parallel(ndev, [&](int i) {
+    return vsg_index_create(g->ctx[static_cast<size_t>(i)], g->db[static_cast<size_t>(i)], wordlength, g->mask_lower,
+                            &g->index[static_cast<size_t>(i)]);
+  });
   g->index_ms = now_ms() - t0;
-  for (int i = 0; i < ndev; i++) {
-    if (rcs[static_cast<size_t>(i)] != VSG_OK) { Error::set(msgs[static_cast<size_t>(i)]); rc = rcs[static_cast<size_t>(i)]; vsg_group_destroy(g); return rc; }
-  }
+  if (rc != VSG_OK) { vsg_group_destroy(g); return rc; }
   *out = g;
   return VSG_OK;
 }
@@ -197,12 +188,10 @@ extern "C" int vsg_group_search(vsg_group * g, const char * qcat, const int64_t 
       while (p < nd && acc >= total * p / nd) { bounds[static_cast<size_t>(p++)] = i + 1; }
     }
   }
-  std::vector<int> rcs(static_cast<size_t>(nd), VSG_OK);
-  std::vector<std::string> msgs(static_cast<size_t>(nd));
   std::vector<int64_t> w(static_cast<size_t>(nd) * 4, 0);
-  auto run = [&](int d) {
+  int const rc = run_parallel(nd, [&](int d) -> int {
     int64_t const b0 = bounds[static_cast<size_t>(d)], b1 = bounds[static_cast<size_t>(d) + 1];
-    if (b1 <= b0) { return; }
+    if (b1 <= b0) { return VSG_OK; }
     vsg_ctx * c = g->ctx[static_cast<size_t>(d)];
     // this device's slice, rebased: offsets relative to its first sequence
     int64_t const base = qoff[b0];
@@ -220,19 +209,13 @@ extern "C" int vsg_group_search(vsg_group * g, const char * qcat, const int64_t 
       rc = vsg_search_batch(c, g->index[static_cast<size_t>(d)], g->db[static_cast<size_t>(d)], q, 0, b1 - b0, &o,
                             results + static_cast<size_t>(b0) * max_results, max_results, counts + b0, w.data() + 4 * d);
     }
-    if (rc != VSG_OK) { rcs[static_cast<size_t>(d)] = rc; msgs[static_cast<size_t>(d)] = vsg_last_error(); }
     if (g->fallback != nullptr) { vsg_ctx_set_fallback(c, g->fallback, g->fallback_user); }
     if (q != nullptr) { vsg_seqset_destroy(q); }
-  };
-  if (nd == 1) { run(0); }
-  else {
-    std::vector<std::thread> pool;
-    for (int d = 0; d < nd; d++) { pool.emplace_back(run, d); }
-    for (auto & th : pool) { th.join(); }
-  }
-  for (int d = 0; d < nd; d++) {
-    if (rcs[static_cast<size_t>(d)] != VSG_OK) { Error::set(msgs[static_cast<size_t>(d)]); return rcs[static_cast<size_t>(d)]; }
-    if (work != nullptr) { for (int z = 0; z < 4; z++) { work[z] += w[static_cast<size_t>(4 * d + z)]; } }
+    return rc;
+  });
+  if (rc != VSG_OK) { return rc; }
+  for (int d = 0; d < nd && work != nullptr; d++) {
+    for (int z = 0; z < 4; z++) { work[z] += w[static_cast<size_t>(4 * d + z)]; }
   }
   return VSG_OK;
 }
@@ -266,26 +249,17 @@ extern "C" int vsg_group_allpairs(vsg_group * g, const vsg_search_opts * opts, v
     }
     cap_off[static_cast<size_t>(nd)] = cap;
   }
-  std::vector<int> rcs(static_cast<size_t>(nd), VSG_OK);
-  std::vector<std::string> msgs(static_cast<size_t>(nd));
   std::vector<int64_t> got(static_cast<size_t>(nd), 0), w(static_cast<size_t>(nd) * 2, 0);
-  auto run = [&](int d) {
+  rc = run_parallel(nd, [&](int d) -> int {
     int64_t const r0 = bounds[static_cast<size_t>(d)], r1 = bounds[static_cast<size_t>(d) + 1];
-    if (r1 <= r0) { return; }
-    int const r = vsg_allpairs(g->ctx[static_cast<size_t>(d)], g->db[static_cast<size_t>(d)], r0, r1 - r0, opts,
-                               hits + cap_off[static_cast<size_t>(d)], cap_off[static_cast<size_t>(d) + 1] - cap_off[static_cast<size_t>(d)],
-                               &got[static_cast<size_t>(d)], w.data() + 2 * d);
-    if (r != VSG_OK) { rcs[static_cast<size_t>(d)] = r; msgs[static_cast<size_t>(d)] = vsg_last_error(); }
-  };
-  if (nd == 1) { run(0); }
-  else {
-    std::vector<std::thread> pool;
-    for (int d = 0; d < nd; d++) { pool.emplace_back(run, d); }
-    for (auto & th : pool) { th.join(); }
-  }
+    if (r1 <= r0) { return VSG_OK; }
+    return vsg_allpairs(g->ctx[static_cast<size_t>(d)], g->db[static_cast<size_t>(d)], r0, r1 - r0, opts,
+                        hits + cap_off[static_cast<size_t>(d)], cap_off[static_cast<size_t>(d) + 1] - cap_off[static_cast<size_t>(d)],
+                        &got[static_cast<size_t>(d)], w.data() + 2 * d);
+  });
+  if (rc != VSG_OK) { return rc; }
   int64_t pos = 0;
   for (int d = 0; d < nd; d++) {
-    if (rcs[static_cast<size_t>(d)] != VSG_OK) { Error::set(msgs[static_cast<size_t>(d)]); return rcs[static_cast<size_t>(d)]; }
     // compact the per-device stretches into one list in row order
     if (cap_off[static_cast<size_t>(d)] != pos && got[static_cast<size_t>(d)] > 0) {
       std::memmove(hits + pos, hits + cap_off[static_cast<size_t>(d)], sizeof(vsg_pair_hit) * static_cast<size_t>(got[static_cast<size_t>(d)]));
