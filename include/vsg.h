@@ -94,6 +94,12 @@ int vsg_seqset_dust(vsg_ctx * ctx, vsg_seqset * s);
 /* the symbol bytes as stored in HBM (bits 0-3 = 4-bit nucleotide code, bit 4 = lower case), in the
  * order and at the offsets given to vsg_seqset_create; cap >= total sequence bytes.  For tools/tests. */
 int vsg_seqset_symbols(vsg_ctx * ctx, const vsg_seqset * s, uint8_t * out, int64_t cap);
+/* reverse_complement (utils/reverse_complement.cpp) of the sequences [q0, q0 + n) of `src`, made on the device into a
+ * new set of n sequences: entry i is the reverse complement of src's sequence q0 + i.  The complement of an IUPAC code
+ * is its complement code, any other byte becomes 'N', and every symbol keeps its case, so a soft mask carries over.
+ * q0 / n must lie inside `src` (n = 0 gives an empty set) and `src` must belong to ctx's device, else VSG_EINVAL.
+ * E.g. the CIGAR of a minus-strand clustering hit is vsg_align_pairs(ctx, rc, set, ...) with rc the whole set's. */
+int vsg_seqset_revcomp(vsg_ctx * ctx, const vsg_seqset * src, int64_t q0, int64_t n, vsg_seqset ** out);
 
 /* ---- batched alignment: replaces search16_qprep + search16 (core/align_simd.cpp:1406-2060)
  *      for npairs (query,target) pairs at once.  qidx[i] indexes `queries`, tidx[i] indexes
@@ -306,9 +312,14 @@ int vsg_allpairs(vsg_ctx * ctx, const vsg_seqset * set, int64_t row0, int64_t nr
  *      --uc) or the sequence number of the centroid it matched plus that alignment's statistics and identity
  *      (an "H" record; the CIGAR is one vsg_align_pairs call away).  NOTE the reference's default --maxrejects for
  *      --cluster_fast is 8, not 32 (cli.cc:4163-4172): set opts->maxrejects accordingly.  opts: id, iddef, maxaccepts, maxrejects,
- *      wordlength, minwordmatches, mask_lower, the length / abundance / post-alignment filters (target_sizes
- *      and target_labels are per sequence of `set`); plus strand only.  work (optional, 2 x int64): pairs and DP
- *      cells handed to the aligner. ---- */
+ *      wordlength, minwordmatches, mask_lower, strand_both, the length / abundance / post-alignment filters (target_sizes
+ *      and target_labels are per sequence of `set`).  strand_both = --strand both (cluster.cpp:162-189, 920-957): every
+ *      sequence is also searched as its reverse complement, which keeps the set's soft mask; strand = 1 marks a hit
+ *      of the reverse complement (the "-" of --uc column 5), whose statistics and CIGAR are those of the reverse-complemented
+ *      sequence against the centroid: vsg_align_pairs(ctx, rc, set, ...) with rc from vsg_seqset_revcomp.  A centroid is
+ *      always its plus strand.  A pair deferred to the fallback callback reaches it as (sequence, strand, centroid).
+ *      The both-strands query set costs 2 bytes of device memory per nucleotide of `set`.  work (optional, 2 x int64):
+ *      pairs and DP cells handed to the aligner, both strands counted. ---- */
 typedef struct vsg_cluster_result {
   int32_t cluster;
   int32_t centroid;

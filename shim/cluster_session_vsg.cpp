@@ -7,12 +7,13 @@
 // forwarding to a vsg_cluster_session of libvsg.so (include/vsg.h): the database is mirrored into HBM once at
 // cluster_session_init, every call ranks / aligns / resolves its range in rounds on the device and the host
 // (vsearch_b200/csrc/cluster.cu), the CIGARs of the assigned sequences come from one vsg_align_pairs call per
-// range.  The caller's Dbindex is not touched: the centroids' k-mer index lives on the device.  Link so that these
-// definitions win over core/cluster.cpp.o's (oracle/Makefile weakens those six symbols).  See INTEGRATION.md.
+// range and strand.  The caller's Dbindex is not touched: the centroids' k-mer index lives on the device.  Link so that
+// these definitions win over core/cluster.cpp.o's (oracle/Makefile weakens those six symbols).  See INTEGRATION.md.
 #include "vsearch_api.h"
 #include "core/cluster.hpp"
 #include "core/linmemalign.hpp"
 #include "utils/fatal.hpp"
+#include "utils/reverse_complement.hpp"
 #include "utils/string_alloc.hpp"
 
 #include "vsg.h"
@@ -44,6 +45,7 @@ struct cluster_session_s {
   int seqcount = 0;
   vsg_ctx * ctx = nullptr;
   vsg_seqset * set = nullptr;
+  vsg_seqset * rc = nullptr;     // --strand both: the reverse complements of `set`, the queries of minus-strand CIGARs
   vsg_cluster_session * session = nullptr;
   vsg_search_opts opts;
   std::vector<int64_t> sizes, labels;
@@ -56,13 +58,20 @@ struct Lma {
   std::string cigar;
   int64_t out[10];
 };
-void lma_align(cluster_session_s const & cs, int64_t query, int64_t target, Lma & r)
+// strand = 1: the query's reverse complement against the target, as cluster_query_core searches it (cluster.cpp:177-183)
+void lma_align(cluster_session_s const & cs, int64_t query, int32_t strand, int64_t target, Lma & r)
 {
   Parameters const & p = *cs.parameters;
-  char const * const q = cs.db->getsequence(static_cast<uint64_t>(query));
+  char const * q = cs.db->getsequence(static_cast<uint64_t>(query));
   char const * const d = cs.db->getsequence(static_cast<uint64_t>(target));
   auto const ql = static_cast<int64_t>(cs.db->getsequencelen(static_cast<uint64_t>(query)));
   auto const dl = static_cast<int64_t>(cs.db->getsequencelen(static_cast<uint64_t>(target)));
+  std::vector<char> q_rc;
+  if (strand != 0) {
+    q_rc.resize(static_cast<size_t>(ql) + 1);
+    reverse_complement(q_rc.data(), q, ql);
+    q = q_rc.data();
+  }
   struct Scoring scoring = scoring_from_options(p);
   LinearMemoryAligner lma(scoring);
   char * const cigar = xstrdup(lma.align(q, d, ql, dl));
@@ -91,10 +100,10 @@ void lma_align(cluster_session_s const & cs, int64_t query, int64_t target, Lma 
   xfree(cigar);
 }
 
-int lma_fallback(void * user, int64_t query, int32_t, int64_t target, int64_t * out)
+int lma_fallback(void * user, int64_t query, int32_t strand, int64_t target, int64_t * out)
 {
   Lma r;
-  lma_align(*static_cast<cluster_session_s *>(user), query, target, r);
+  lma_align(*static_cast<cluster_session_s *>(user), query, strand, target, r);
   std::memcpy(out, r.out, sizeof r.out);
   return 0;
 }
@@ -113,25 +122,34 @@ void assign_range(cluster_session_s * cs, int start, int count, int round_size, 
   }
   std::vector<vsg_cluster_result> r(static_cast<size_t>(count));
   if (vsg_cluster_session_assign(cs->session, start, count, round_size, r.data()) != VSG_OK) { die("vsg_cluster_session_assign"); }
-  // CIGARs of the assigned sequences: one batched call
-  std::vector<uint32_t> q, t;
-  std::vector<int> who;
-  int64_t cap = 64;
+  // CIGARs of the assigned sequences: one batched call per strand, the minus strand's with the reverse complements as
+  // queries (the reference keeps the CIGAR of the reverse-complemented query, cluster.cpp:978-991)
+  struct StrandPairs {
+    std::vector<uint32_t> q, t;
+    int64_t cap = 64;
+    std::vector<int16_t> sc;
+    std::vector<char> cig;
+    std::vector<int64_t> coff;
+    size_t next = 0;
+  } sp[2];
   for (int i = 0; i < count; i++) {
-    if (r[static_cast<size_t>(i)].centroid >= 0) {
-      q.push_back(static_cast<uint32_t>(start + i)); t.push_back(static_cast<uint32_t>(r[static_cast<size_t>(i)].centroid));
-      who.push_back(i);
-      cap += static_cast<int64_t>(cs->db->getsequencelen(static_cast<uint64_t>(start + i))) +
-             static_cast<int64_t>(cs->db->getsequencelen(static_cast<uint64_t>(r[static_cast<size_t>(i)].centroid))) + 1;
+    vsg_cluster_result const & x = r[static_cast<size_t>(i)];
+    if (x.centroid >= 0) {
+      StrandPairs & s = sp[x.strand != 0 ? 1 : 0];
+      s.q.push_back(static_cast<uint32_t>(start + i)); s.t.push_back(static_cast<uint32_t>(x.centroid));
+      s.cap += static_cast<int64_t>(cs->db->getsequencelen(static_cast<uint64_t>(start + i))) +
+               static_cast<int64_t>(cs->db->getsequencelen(static_cast<uint64_t>(x.centroid))) + 1;
     }
   }
-  size_t const np = q.size();
-  std::vector<int16_t> sc(np); std::vector<uint16_t> al(np), ma(np), mi(np), ga(np);
-  std::vector<char> cig(static_cast<size_t>(cap));
-  std::vector<int64_t> coff(np + 1);
-  if (np > 0 && vsg_align_pairs(cs->ctx, cs->set, cs->set, static_cast<int64_t>(np), q.data(), t.data(), sc.data(), al.data(), ma.data(),
-                                mi.data(), ga.data(), nullptr, cig.data(), cap, coff.data()) != VSG_OK) { die("vsg_align_pairs"); }
-  size_t pi = 0;
+  for (int strand = 0; strand < 2; strand++) {
+    StrandPairs & s = sp[strand];
+    size_t const np = s.q.size();
+    if (np == 0) { continue; }
+    std::vector<uint16_t> al(np), ma(np), mi(np), ga(np);
+    s.sc.resize(np); s.cig.resize(static_cast<size_t>(s.cap)); s.coff.resize(np + 1);
+    if (vsg_align_pairs(cs->ctx, strand != 0 ? cs->rc : cs->set, cs->set, static_cast<int64_t>(np), s.q.data(), s.t.data(), s.sc.data(),
+                        al.data(), ma.data(), mi.data(), ga.data(), nullptr, s.cig.data(), s.cap, s.coff.data()) != VSG_OK) { die("vsg_align_pairs"); }
+  }
   for (int i = 0; i < count; i++) {
     cluster_result_s & out = results[i];
     std::memset(&out, 0, sizeof out);
@@ -147,12 +165,13 @@ void assign_range(cluster_session_s * cs, int start, int count, int round_size, 
       out.centroid_seqno = x.centroid;
       out.identity = x.id;
       label_into(out.centroid_label, *cs->db, x.centroid);
+      StrandPairs & s = sp[x.strand != 0 ? 1 : 0];
+      size_t const pi = s.next++;
       std::string text;
-      if (sc[pi] == SHRT_MAX) { Lma l; lma_align(*cs, start + i, x.centroid, l); text = l.cigar; }   // the deferred pair's CIGAR
-      else { text = cig.data() + coff[pi]; }
+      if (s.sc[pi] == SHRT_MAX) { Lma l; lma_align(*cs, start + i, x.strand, x.centroid, l); text = l.cigar; }   // the deferred pair's CIGAR
+      else { text = s.cig.data() + s.coff[pi]; }
       int const n = std::snprintf(out.cigar, sizeof out.cigar, "%s", text.c_str());
       out.cigar_truncated = (n >= static_cast<int>(sizeof out.cigar));
-      ++pi;
     }
   }
 }
@@ -165,6 +184,7 @@ auto cluster_session_cleanup(struct cluster_session_s * cs) -> void
 {
   if (cs == nullptr) { return; }
   if (cs->session != nullptr) { vsg_cluster_session_destroy(cs->session); cs->session = nullptr; }
+  if (cs->rc != nullptr) { vsg_seqset_destroy(cs->rc); cs->rc = nullptr; }
   if (cs->set != nullptr) { vsg_seqset_destroy(cs->set); cs->set = nullptr; }
   if (cs->ctx != nullptr) { vsg_ctx_destroy(cs->ctx); cs->ctx = nullptr; }
 }
@@ -181,7 +201,6 @@ auto cluster_session_init(struct cluster_session_s * cs, struct Parameters const
   Parameters const & p = parameters;
   cs->parameters = &p; cs->dbindex = &dbindex; cs->db = &db;
   cs->seqcount = static_cast<int>(db.getsequencecount());
-  if (p.opt_strand) { fatal("GPU cluster session: --strand both is not offered on this path"); }
 
   vsg_scoring sco;
   int64_t const v[14] = {p.opt_match, p.opt_mismatch,
@@ -211,6 +230,7 @@ auto cluster_session_init(struct cluster_session_s * cs, struct Parameters const
     cs->labels[i] = it.first->second;
   }
   if (vsg_seqset_create(cs->ctx, cat.data(), off.data(), len.data(), static_cast<int64_t>(n), 1, &cs->set) != VSG_OK) { die("vsg_seqset_create"); }
+  if (p.opt_strand && vsg_seqset_revcomp(cs->ctx, cs->set, 0, static_cast<int64_t>(n), &cs->rc) != VSG_OK) { die("vsg_seqset_revcomp"); }
 
   vsg_search_opts & o = cs->opts;
   vsg_search_opts_default(&o);
@@ -220,6 +240,7 @@ auto cluster_session_init(struct cluster_session_s * cs, struct Parameters const
   o.minwordmatches = static_cast<int32_t>(p.opt_minwordmatches);
   o.iddef = static_cast<int32_t>(p.opt_iddef);
   o.mask_lower = (p.opt_qmask != Masking::none) ? 1 : 0;
+  o.strand_both = p.opt_strand ? 1 : 0;
   o.minqt = p.opt_minqt; o.maxqt = p.opt_maxqt; o.minsl = p.opt_minsl; o.maxsl = p.opt_maxsl;
   o.maxid = p.opt_maxid; o.mid = p.opt_mid; o.query_cov = p.opt_query_cov; o.target_cov = p.opt_target_cov;
   o.maxsubs = p.opt_maxsubs; o.maxgaps = p.opt_maxgaps; o.mincols = p.opt_mincols; o.maxdiffs = p.opt_maxdiffs;

@@ -831,6 +831,29 @@ __global__ void revcomp_kernel(DevSeqs src, int64_t q0, int64_t n, const int64_t
   }
 }
 
+// both strands of every sequence of `src`, interleaved: sequence s is copied to dst_off[2s] and its reverse
+// complement (as revcomp_kernel: bit-reversed code, non-IUPAC -> 'N', case kept) written to dst_off[2s+1].
+// One warp per source sequence.
+__global__ void both_strands_kernel(DevSeqs src, const int64_t * __restrict__ dst_off, uint8_t * __restrict__ dst)
+{
+  int64_t const w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  int const lane = threadIdx.x & 31;
+  if (w >= src.n) { return; }
+  uint8_t const * p = src.sym + src.off[w];
+  int const len = src.len[w];
+  uint8_t * plus = dst + dst_off[2 * w];
+  uint8_t * minus = dst + dst_off[2 * w + 1];
+  for (int i = lane; i < len; i += 32) {
+    int const s = p[i];
+    plus[i] = static_cast<uint8_t>(s);
+    int const c = s & 15;
+    int r;
+    if (c == 0) { r = 15; }
+    else { r = ((c & 1) << 3) | ((c & 2) << 1) | ((c & 4) >> 1) | ((c & 8) >> 3); r |= (s & 16); }
+    minus[len - 1 - i] = static_cast<uint8_t>(r);
+  }
+}
+
 __global__ void nonacgt_kernel(DevSeqs s, uint8_t * __restrict__ flag)
 {
   int64_t const w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;

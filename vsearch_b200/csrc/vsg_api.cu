@@ -424,7 +424,63 @@ int seqset_revcomp(vsg_ctx * c, const vsg_seqset * src, int64_t q0, int64_t n, v
   *out = guard.release();
   return VSG_OK;
 }
+
+// Both strands of every sequence of `src` as one compact set of 2n sequences: entry 2s is sequence s, entry 2s+1 its
+// reverse complement.  Made on the device from src's symbols, so a soft mask applied there carries over (the reverse
+// complement keeps the case of each symbol).  The strands of consecutive sequences are consecutive entries.
+int seqset_both_strands(vsg_ctx * c, const vsg_seqset * src, vsg_seqset ** out)
+{
+  *out = nullptr;
+  vsg_seqset * s = new (std::nothrow) vsg_seqset();
+  if (s == nullptr) { Error::set("out of host memory"); return VSG_ENOMEM; }
+  SeqsetGuard guard{s};
+  int64_t const n = src->d.n, n2 = 2 * n;
+  s->device = c->device;
+  s->h_len.resize(static_cast<size_t>(n2));
+  s->h_nonacgt.resize(static_cast<size_t>(n2));
+  std::vector<int64_t> h_off(static_cast<size_t>(n2));
+  int64_t total = 0;
+  for (int64_t i = 0; i < n2; i++) {
+    size_t const from = static_cast<size_t>(i >> 1);
+    s->h_len[static_cast<size_t>(i)] = src->h_len[from];
+    s->h_nonacgt[static_cast<size_t>(i)] = src->h_nonacgt[from];
+    h_off[static_cast<size_t>(i)] = total;
+    total += src->h_len[from];
+  }
+  s->total = total;
+  s->h_off = h_off;
+  int rc;
+  if ((rc = s->b_sym.reserve(static_cast<size_t>(total) + 64)) != VSG_OK ||
+      (rc = s->b_off.reserve(sizeof(int64_t) * static_cast<size_t>(n2) + 8)) != VSG_OK ||
+      (rc = s->b_len.reserve(sizeof(int32_t) * static_cast<size_t>(n2) + 8)) != VSG_OK) {
+    return rc;
+  }
+  s->d.sym = static_cast<uint8_t *>(s->b_sym.p);
+  s->d.off = static_cast<int64_t *>(s->b_off.p);
+  s->d.len = static_cast<int32_t *>(s->b_len.p);
+  s->d.n = n2;
+  if (n > 0) {
+    VSG_CUDA_OK(cudaMemcpyAsync(s->b_off.p, h_off.data(), sizeof(int64_t) * n2, cudaMemcpyHostToDevice, c->stream));
+    VSG_CUDA_OK(cudaMemcpyAsync(s->b_len.p, s->h_len.data(), sizeof(int32_t) * n2, cudaMemcpyHostToDevice, c->stream));
+    int64_t const blocks = (n * 32 + 255) / 256;
+    both_strands_kernel<<<static_cast<unsigned>(blocks), 256, 0, c->stream>>>(src->d, s->d.off, static_cast<uint8_t *>(s->b_sym.p));
+    count_launch();
+    VSG_CUDA_OK(cudaStreamSynchronize(c->stream));  // h_off goes out of scope
+  }
+  *out = guard.release();
+  return VSG_OK;
+}
 }  // namespace vsg
+
+extern "C" int vsg_seqset_revcomp(vsg_ctx * c, const vsg_seqset * src, int64_t q0, int64_t n, vsg_seqset ** out)
+{
+  if (c == nullptr || src == nullptr || out == nullptr) { Error::set("vsg_seqset_revcomp: null argument"); return VSG_EINVAL; }
+  *out = nullptr;
+  if (q0 < 0 || n < 0 || q0 > src->d.n || n > src->d.n - q0) { Error::set("vsg_seqset_revcomp: range outside the sequence set"); return VSG_EINVAL; }
+  if (src->device != c->device) { Error::set("vsg_seqset_revcomp: the sequence set lives on another device than the context"); return VSG_EINVAL; }
+  VSG_CUDA_OK(cudaSetDevice(c->device));
+  return seqset_revcomp(c, src, q0, n, out);
+}
 
 extern "C" int64_t vsg_seqset_count(const vsg_seqset * s) { return s != nullptr ? s->d.n : 0; }
 

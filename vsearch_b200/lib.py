@@ -234,6 +234,16 @@ class Context:
                                         C.c_int64(n), C.c_int(0), C.byref(h)), "vsg_seqset_create")
         return SeqSetHandle(self, h, n, None)
 
+    def revcomp(self, ss: SeqSetHandle, q0: int = 0, n: Optional[int] = None) -> SeqSetHandle:
+        """vsg_seqset_revcomp: the reverse complements of sequences [q0, q0 + n) of `ss` (default: to the end) as a
+        new set, made on the device; the case (soft mask) of every symbol is kept."""
+        if n is None:
+            n = ss.n - q0
+        h = C.c_void_p()
+        _check(load().vsg_seqset_revcomp(self.h, ss.h, C.c_int64(q0), C.c_int64(n), C.byref(h)), "vsg_seqset_revcomp")
+        lens = ss.lens[q0:q0 + n] if ss.lens is not None else None
+        return SeqSetHandle(self, h, n, lens)
+
     def align_pairs(self, qs: SeqSetHandle, ts: SeqSetHandle, qidx: np.ndarray, tidx: np.ndarray,
                     cigar: bool = False) -> AlignResult:
         lib = load()
