@@ -531,7 +531,7 @@ traceback_ckpt_tasks_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, 
   else { traceback_ckpt_tasks_body<RT, false>(sp, qs, ts, tasks, ntasks, R, rowck, colck, stats, gate, tb_smem); }
 }
 
-// with CIGAR text, from pair descriptors (kind 2 = checkpoint layout; the others belong to traceback_kernel)
+// with CIGAR text, from pair descriptors (PD_CKPT = checkpoint layout; the others belong to traceback_kernel)
 template <int RT>
 __global__ void __launch_bounds__(TB_CK_THREADS)
 traceback_ckpt_pairs_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, DevSeqs ts,
@@ -543,7 +543,7 @@ traceback_ckpt_pairs_kernel(const __grid_constant__ ScoreParams sp, DevSeqs qs, 
   int const p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= npairs) { return; }
   PairDesc const pd = pairs[p];
-  if (pd.kind != 2 || (RT == 8) != (pd.R <= 8)) { return; }
+  if (pd.kind != PD_CKPT || (RT == 8) != (pd.R <= 8)) { return; }
   traceback_ckpt_one<RT, true>(sp, qs, ts, pd.q, pd.t, pd.out, pd.R, pd.half & 1, pd.half >> 1,
                                rowck + pd.dir_off, colck + pd.aux_off, cigar_scratch + pd.cigar_off, stats, tb_smem);
 }

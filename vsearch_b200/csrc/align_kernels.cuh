@@ -523,7 +523,7 @@ struct DirReader {
   uint4 tile = {0u, 0u, 0u, 0u};
   __device__ __forceinline__ void start(int i)
   {
-    if (kind == 1) { row_base = static_cast<size_t>(i) * D; return; }
+    if (kind == PD_EXACT) { row_base = static_cast<size_t>(i) * D; return; }
     int const strip = i / strip_rows;
     int const il = i - strip * strip_rows;
     l = il / R;
@@ -533,7 +533,7 @@ struct DirReader {
   }
   __device__ __forceinline__ void up()  // i -> i - 1
   {
-    if (kind == 1) { row_base -= static_cast<size_t>(D); return; }
+    if (kind == PD_EXACT) { row_base -= static_cast<size_t>(D); return; }
     if (--r < 0) {
       r = R - 1;
       if (--l < 0) { l = 31; row_base -= strip_bytes; }
@@ -541,7 +541,7 @@ struct DirReader {
   }
   __device__ __forceinline__ int get(int j)
   {
-    if (kind == 1) { return base[row_base + j]; }
+    if (kind == PD_EXACT) { return base[row_base + j]; }
     int const sg = j + l;  // wavefront step at which lane l visits column j
     int const g = sg >> sh;
     size_t const a = row_base + (static_cast<size_t>(g) * 32 + l) * 16;
@@ -722,7 +722,7 @@ __global__ void traceback_kernel(const __grid_constant__ ScoreParams sp, DevSeqs
   int const p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= npairs) { return; }
   PairDesc const pd = pairs[p];
-  if (pd.kind == 2) { return; }  // checkpoint layout: traceback_ckpt_pairs_kernel's (align_ckpt.cuh)
+  if (pd.kind == PD_CKPT) { return; }  // checkpoint layout: traceback_ckpt_pairs_kernel's (align_ckpt.cuh)
   traceback_one<TEXT>(sp, qs, ts, pd, dir, cigar_scratch, stats);
 }
 
@@ -739,7 +739,7 @@ __global__ void traceback_fast_tasks_kernel(const __grid_constant__ ScoreParams 
   int const out = half ? tk.out_hi : tk.out_lo;
   if (out < 0) { return; }
   PairDesc pd;
-  pd.q = tk.q; pd.t = half ? tk.thi : tk.tlo; pd.dir_off = tk.dir_off; pd.kind = 0; pd.out = out;
+  pd.q = tk.q; pd.t = half ? tk.thi : tk.tlo; pd.dir_off = tk.dir_off; pd.kind = PD_FAST; pd.out = out;
   pd.R = R; pd.half = half; pd.dmax = tk.dmax; pd.cigar_off = 0;
   traceback_one<false>(sp, qs, ts, pd, dir, nullptr, stats);
 }
@@ -752,7 +752,7 @@ __global__ void traceback_exact_tasks_kernel(const __grid_constant__ ScoreParams
   if (id >= ntasks) { return; }
   ExactTask const tk = tasks[id];
   PairDesc pd;
-  pd.q = tk.q; pd.t = tk.t; pd.dir_off = tk.dir_off; pd.kind = 1; pd.out = tk.out;
+  pd.q = tk.q; pd.t = tk.t; pd.dir_off = tk.dir_off; pd.kind = PD_EXACT; pd.out = tk.out;
   pd.R = 1; pd.half = 0; pd.dmax = 0; pd.cigar_off = 0;
   traceback_one<false>(sp, qs, ts, pd, dir, nullptr, stats);
 }

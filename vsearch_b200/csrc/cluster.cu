@@ -35,7 +35,6 @@ int cindex_append(vsg_ctx * c, CIndex * ix, const uint32_t * seqnos, int n);
 int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
                         int tophits, uint32_t ** d_seqno, uint32_t ** d_count, int32_t ** d_n, int32_t ** d_status);
 const std::vector<uint32_t> & cindex_seqnos(const CIndex * ix);
-int seqset_both_strands(vsg_ctx * c, const vsg_seqset * src, vsg_seqset ** out);
 }  // namespace vsg
 
 using namespace vsg;
@@ -92,7 +91,7 @@ struct vsg_cluster_session {
   // The query strands: `set` itself, or with --strand both a set of 2 * seqcount entries made at setup, sequence s at
   // 2s and its reverse complement at 2s+1, so that the strands of a round are one contiguous range.
   const vsg_seqset * qset = nullptr;
-  vsg_seqset * both = nullptr;                     // owned
+  vsg::SeqsetPtr both;
   int nstrands = 1;
   vsg_search_opts opts;
   vsg::SearchLimits lim{};
@@ -107,7 +106,6 @@ struct vsg_cluster_session {
   ~vsg_cluster_session()
   {
     if (ix != nullptr) { cindex_destroy(ix); }
-    if (both != nullptr) { vsg_seqset_destroy(both); }
   }
 };
 
@@ -138,8 +136,8 @@ int session_setup(vsg_ctx * c, const vsg_seqset * set, const vsg_search_opts * o
   if (opts->strand_both != 0) {
     // the reverse complements keep the soft mask of the plus strands (cluster.cpp:162-189 reverse-complements the
     // dust_all'ed database sequence and does not mask it again)
-    if (int const r = seqset_both_strands(c, set, &s.both); r != VSG_OK) { return r; }
-    s.qset = s.both;
+    if (int const r = seqset_both_strands(c, set, s.both); r != VSG_OK) { return r; }
+    s.qset = s.both.get();
     s.nstrands = 2;
   }
   return cindex_create(c, set, k, opts->mask_lower, &s.ix);

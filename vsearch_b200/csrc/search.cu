@@ -28,7 +28,6 @@ namespace vsg {
 int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
                  int minwordmatches, int tophits, int mask_lower, uint32_t ** d_seqno, uint32_t ** d_count,
                  int32_t ** d_n, int32_t ** d_status);
-int seqset_revcomp(vsg_ctx * c, const vsg_seqset * src, int64_t q0, int64_t nq, vsg_seqset ** out);
 void rank_collect_time(vsg_ctx * c);
 const vsg_seqset * index_db(const vsg_index * ix);
 int index_wordlength(const vsg_index * ix);
@@ -207,21 +206,20 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
   {
 
     int64_t const bn = std::min(bn_req, nq - b0);
-    vsg_seqset * rc_set = nullptr;
-    struct RcGuard { vsg_seqset *& s; ~RcGuard() { if (s != nullptr) { vsg_seqset_destroy(s); s = nullptr; } } } rc_guard{rc_set};   // every exit
+    SeqsetPtr rc_set;
     if (nstrands == 2) {
-      int r = seqset_revcomp(c, queries, q0 + b0, bn, &rc_set);
+      int r = seqset_revcomp(c, queries, q0 + b0, bn, rc_set);
       if (r != VSG_OK) { return r; }
       // each strand is masked on its own (search.cpp:437-449); dust() upper-cases first, so the case the
       // reverse complement inherited from the masked plus strand does not matter
-      if (opts->qmask_dust != 0 && (r = vsg_seqset_dust(c, rc_set)) != VSG_OK) { return r; }
+      if (opts->qmask_dust != 0 && (r = vsg_seqset_dust(c, rc_set.get())) != VSG_OK) { return r; }
     }
     size_t const cells = static_cast<size_t>(bn) * tophits;
     sc.h_seqno.resize(cells * nstrands); sc.h_count.resize(cells * nstrands); sc.h_n.resize(static_cast<size_t>(bn) * nstrands);
     if (content_filters) { sc.h_flags.resize(cells * nstrands); }
     for (int s = 0; s < nstrands; s++) {
       uint32_t *d_seqno, *d_count; int32_t *d_n, *d_status;
-      const vsg_seqset * qset = (s == 0) ? queries : rc_set;
+      const vsg_seqset * qset = (s == 0) ? queries : rc_set.get();
       int64_t const qq0 = (s == 0) ? q0 + b0 : 0;
       int r = rank_enqueue(c, ix, qset, qq0, bn, lim.minwordmatches, tophits, opts->mask_lower, &d_seqno, &d_count, &d_n, &d_status);
       if (r != VSG_OK) { return r; }
@@ -391,7 +389,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
         for (int part = 0; part < 2; part++) {
           size_t const lo = part == 0 ? 0 : split, hi = part == 0 ? split : n;
           if (hi <= lo) { continue; }
-          const vsg_seqset * qset = part == 0 ? queries : rc_set;
+          const vsg_seqset * qset = part == 0 ? queries : rc_set.get();
           const int32_t * lead_part = nullptr;
           if (lead != nullptr) {
             // leaders as indices into this part's own pair list (a group never straddles the strands)
@@ -486,7 +484,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
             if (gated_round && plead[i] >= 0 && a.walk_skipped(i)) {
               // its walk was skipped because the device took the group's leader for accepted, yet the replay is here:
               // the two verdicts differ (a borderline identity); align this pair now
-              int const r = align_into(c, S.strand == 0 ? queries : rc_set, db, 1, &pq[i], &pt[i], a, i);
+              int const r = align_into(c, S.strand == 0 ? queries : rc_set.get(), db, 1, &pq[i], &pt[i], a, i);
               if (r != VSG_OK) { return r; }
               tb_redone++;
             }

@@ -101,7 +101,6 @@ void PinBuf::release() { if (p != nullptr) { cudaFreeHost(p); p = nullptr; cap =
 // scope guards for the error paths (VSG_CUDA_OK returns from the middle of a function)
 namespace {
 struct ScopedBuf { DevBuf b; ~ScopedBuf() { b.release(); } };
-struct SeqsetGuard { vsg_seqset * s; ~SeqsetGuard() { if (s != nullptr) { vsg_seqset_destroy(s); } } vsg_seqset * release() { vsg_seqset * r = s; s = nullptr; return r; } };
 struct CtxGuard { vsg_ctx * c; ~CtxGuard() { if (c != nullptr) { vsg_ctx_destroy(c); } } vsg_ctx * release() { vsg_ctx * r = c; c = nullptr; return r; } };
 }  // namespace
 
@@ -301,6 +300,39 @@ extern "C" int vsg_ctx_sync(vsg_ctx * c)
 }
 
 // ---- sequence sets ---------------------------------------------------------------------------
+namespace {
+// A set of len.size() sequences at the given offsets (symbols: `total` bytes) on c's device, with the device copies of
+// offsets and lengths under way on c's stream; the caller writes the symbols.
+int seqset_alloc(vsg_ctx * c, std::vector<int32_t> len, std::vector<int64_t> off, int64_t total,
+                 std::vector<uint8_t> nonacgt, SeqsetPtr & out)
+{
+  SeqsetPtr s(new (std::nothrow) vsg_seqset());
+  if (s == nullptr) { Error::set("out of host memory"); return VSG_ENOMEM; }
+  size_t const n = len.size();
+  s->device = c->device;
+  s->h_len = std::move(len);
+  s->h_off = std::move(off);
+  s->h_nonacgt = std::move(nonacgt);
+  s->total = total;
+  int rc;
+  if ((rc = s->b_sym.reserve(static_cast<size_t>(total) + 64)) != VSG_OK ||
+      (rc = s->b_off.reserve(sizeof(int64_t) * n + 8)) != VSG_OK ||
+      (rc = s->b_len.reserve(sizeof(int32_t) * n + 8)) != VSG_OK) {
+    return rc;
+  }
+  s->d.sym = static_cast<uint8_t *>(s->b_sym.p);
+  s->d.off = static_cast<int64_t *>(s->b_off.p);
+  s->d.len = static_cast<int32_t *>(s->b_len.p);
+  s->d.n = static_cast<int64_t>(n);
+  if (n > 0) {
+    VSG_CUDA_OK(cudaMemcpyAsync(s->b_off.p, s->h_off.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, c->stream));
+    VSG_CUDA_OK(cudaMemcpyAsync(s->b_len.p, s->h_len.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, c->stream));
+  }
+  out = std::move(s);
+  return VSG_OK;
+}
+}  // namespace
+
 extern "C" int vsg_seqset_create(vsg_ctx * c, const char * cat, const int64_t * off, const int32_t * len,
                                  int64_t n, int host, vsg_seqset ** out)
 {
@@ -310,35 +342,26 @@ extern "C" int vsg_seqset_create(vsg_ctx * c, const char * cat, const int64_t * 
   }
   *out = nullptr;
   VSG_CUDA_OK(cudaSetDevice(c->device));
-  vsg_seqset * s = new (std::nothrow) vsg_seqset();
-  if (s == nullptr) { Error::set("out of host memory"); return VSG_ENOMEM; }
-  SeqsetGuard guard{s};   // destroys s on every early return
-  s->device = c->device;
-  s->h_len.resize(static_cast<size_t>(n));
+  std::vector<int32_t> h_len(static_cast<size_t>(n));
   std::vector<int64_t> h_off(static_cast<size_t>(n));
   if (host != 0) {
     if (n > 0) {
-      std::memcpy(s->h_len.data(), len, sizeof(int32_t) * static_cast<size_t>(n));
+      std::memcpy(h_len.data(), len, sizeof(int32_t) * static_cast<size_t>(n));
       std::memcpy(h_off.data(), off, sizeof(int64_t) * static_cast<size_t>(n));
     }
   } else if (n > 0) {
-    VSG_CUDA_OK(cudaMemcpyAsync(s->h_len.data(), len, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c->stream));
+    VSG_CUDA_OK(cudaMemcpyAsync(h_len.data(), len, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, c->stream));
     VSG_CUDA_OK(cudaMemcpyAsync(h_off.data(), off, sizeof(int64_t) * n, cudaMemcpyDeviceToHost, c->stream));
     VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
   }
   int64_t total = 0;
   for (int64_t i = 0; i < n; i++) {
-    if (s->h_len[i] < 0 || h_off[i] < 0) { Error::set("vsg_seqset_create: negative length/offset"); return VSG_EINVAL; }
-    total = std::max<int64_t>(total, h_off[i] + s->h_len[i]);
+    if (h_len[i] < 0 || h_off[i] < 0) { Error::set("vsg_seqset_create: negative length/offset"); return VSG_EINVAL; }
+    total = std::max<int64_t>(total, h_off[i] + h_len[i]);
   }
-  s->total = total;
-  s->h_off = h_off;
-  int rc;
-  if ((rc = s->b_sym.reserve(static_cast<size_t>(total) + 64)) != VSG_OK ||
-      (rc = s->b_off.reserve(sizeof(int64_t) * static_cast<size_t>(n) + 8)) != VSG_OK ||
-      (rc = s->b_len.reserve(sizeof(int32_t) * static_cast<size_t>(n) + 8)) != VSG_OK) {
-    return rc;
-  }
+  SeqsetPtr s;
+  int rc = seqset_alloc(c, std::move(h_len), std::move(h_off), total, std::vector<uint8_t>(static_cast<size_t>(n), 0), s);
+  if (rc != VSG_OK) { return rc; }
   const char * d_ascii = cat;
   ScopedBuf tmp_ascii_g;
   DevBuf & tmp_ascii = tmp_ascii_g.b;
@@ -347,15 +370,6 @@ extern "C" int vsg_seqset_create(vsg_ctx * c, const char * cat, const int64_t * 
     VSG_CUDA_OK(cudaMemcpyAsync(tmp_ascii.p, cat, static_cast<size_t>(total), cudaMemcpyHostToDevice, c->stream));
     d_ascii = static_cast<const char *>(tmp_ascii.p);
   }
-  if (n > 0) {
-    VSG_CUDA_OK(cudaMemcpyAsync(s->b_off.p, h_off.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, c->stream));
-    VSG_CUDA_OK(cudaMemcpyAsync(s->b_len.p, s->h_len.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, c->stream));
-  }
-  s->d.sym = static_cast<uint8_t *>(s->b_sym.p);
-  s->d.off = static_cast<int64_t *>(s->b_off.p);
-  s->d.len = static_cast<int32_t *>(s->b_len.p);
-  s->d.n = n;
-  s->h_nonacgt.assign(static_cast<size_t>(n), 0);
   if (total > 0) {
     int64_t const blocks = (total + 255) / 256;
     encode_kernel<<<static_cast<unsigned>(blocks), 256, 0, c->stream>>>(d_ascii, static_cast<uint8_t *>(s->b_sym.p), total);
@@ -376,7 +390,7 @@ extern "C" int vsg_seqset_create(vsg_ctx * c, const char * cat, const int64_t * 
   }
   tmp_ascii.release();
   VSG_CUDA_OK(cudaGetLastError());
-  *out = guard.release();
+  *out = s.release();
   return VSG_OK;
 }
 
@@ -389,85 +403,53 @@ extern "C" void vsg_seqset_destroy(vsg_seqset * s)
 }
 
 namespace vsg {
-int seqset_revcomp(vsg_ctx * c, const vsg_seqset * src, int64_t q0, int64_t n, vsg_seqset ** out)
+int seqset_revcomp(vsg_ctx * c, const vsg_seqset * src, int64_t q0, int64_t n, SeqsetPtr & out)
 {
-  *out = nullptr;
-  vsg_seqset * s = new (std::nothrow) vsg_seqset();
-  if (s == nullptr) { Error::set("out of host memory"); return VSG_ENOMEM; }
-  SeqsetGuard guard{s};
-  s->device = c->device;
-  s->h_len.assign(src->h_len.begin() + q0, src->h_len.begin() + q0 + n);
-  s->h_nonacgt.assign(src->h_nonacgt.begin() + q0, src->h_nonacgt.begin() + q0 + n);
+  std::vector<int32_t> h_len(src->h_len.begin() + q0, src->h_len.begin() + q0 + n);
   std::vector<int64_t> h_off(static_cast<size_t>(n));
   int64_t total = 0;
-  for (int64_t i = 0; i < n; i++) { h_off[static_cast<size_t>(i)] = total; total += s->h_len[static_cast<size_t>(i)]; }
-  s->total = total;
-  s->h_off = h_off;
-  int rc;
-  if ((rc = s->b_sym.reserve(static_cast<size_t>(total) + 64)) != VSG_OK ||
-      (rc = s->b_off.reserve(sizeof(int64_t) * static_cast<size_t>(n) + 8)) != VSG_OK ||
-      (rc = s->b_len.reserve(sizeof(int32_t) * static_cast<size_t>(n) + 8)) != VSG_OK) {
+  for (int64_t i = 0; i < n; i++) { h_off[static_cast<size_t>(i)] = total; total += h_len[static_cast<size_t>(i)]; }
+  SeqsetPtr s;
+  if (int const rc = seqset_alloc(c, std::move(h_len), std::move(h_off), total,
+                                  std::vector<uint8_t>(src->h_nonacgt.begin() + q0, src->h_nonacgt.begin() + q0 + n), s); rc != VSG_OK) {
     return rc;
   }
-  s->d.sym = static_cast<uint8_t *>(s->b_sym.p);
-  s->d.off = static_cast<int64_t *>(s->b_off.p);
-  s->d.len = static_cast<int32_t *>(s->b_len.p);
-  s->d.n = n;
   if (n > 0) {
-    VSG_CUDA_OK(cudaMemcpyAsync(s->b_off.p, h_off.data(), sizeof(int64_t) * n, cudaMemcpyHostToDevice, c->stream));
-    VSG_CUDA_OK(cudaMemcpyAsync(s->b_len.p, s->h_len.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, c->stream));
     int64_t const blocks = (n * 32 + 255) / 256;
     revcomp_kernel<<<static_cast<unsigned>(blocks), 256, 0, c->stream>>>(src->d, q0, n, s->d.off, static_cast<uint8_t *>(s->b_sym.p));
     count_launch();
-    VSG_CUDA_OK(cudaStreamSynchronize(c->stream));  // h_off goes out of scope
+    VSG_CUDA_OK(cudaStreamSynchronize(c->stream));  // the kernel reads src, which the caller may release once this returns
   }
-  *out = guard.release();
+  out = std::move(s);
   return VSG_OK;
 }
 
 // Both strands of every sequence of `src` as one compact set of 2n sequences: entry 2s is sequence s, entry 2s+1 its
 // reverse complement.  Made on the device from src's symbols, so a soft mask applied there carries over (the reverse
 // complement keeps the case of each symbol).  The strands of consecutive sequences are consecutive entries.
-int seqset_both_strands(vsg_ctx * c, const vsg_seqset * src, vsg_seqset ** out)
+int seqset_both_strands(vsg_ctx * c, const vsg_seqset * src, SeqsetPtr & out)
 {
-  *out = nullptr;
-  vsg_seqset * s = new (std::nothrow) vsg_seqset();
-  if (s == nullptr) { Error::set("out of host memory"); return VSG_ENOMEM; }
-  SeqsetGuard guard{s};
   int64_t const n = src->d.n, n2 = 2 * n;
-  s->device = c->device;
-  s->h_len.resize(static_cast<size_t>(n2));
-  s->h_nonacgt.resize(static_cast<size_t>(n2));
+  std::vector<int32_t> h_len(static_cast<size_t>(n2));
+  std::vector<uint8_t> h_nonacgt(static_cast<size_t>(n2));
   std::vector<int64_t> h_off(static_cast<size_t>(n2));
   int64_t total = 0;
   for (int64_t i = 0; i < n2; i++) {
     size_t const from = static_cast<size_t>(i >> 1);
-    s->h_len[static_cast<size_t>(i)] = src->h_len[from];
-    s->h_nonacgt[static_cast<size_t>(i)] = src->h_nonacgt[from];
+    h_len[static_cast<size_t>(i)] = src->h_len[from];
+    h_nonacgt[static_cast<size_t>(i)] = src->h_nonacgt[from];
     h_off[static_cast<size_t>(i)] = total;
     total += src->h_len[from];
   }
-  s->total = total;
-  s->h_off = h_off;
-  int rc;
-  if ((rc = s->b_sym.reserve(static_cast<size_t>(total) + 64)) != VSG_OK ||
-      (rc = s->b_off.reserve(sizeof(int64_t) * static_cast<size_t>(n2) + 8)) != VSG_OK ||
-      (rc = s->b_len.reserve(sizeof(int32_t) * static_cast<size_t>(n2) + 8)) != VSG_OK) {
-    return rc;
-  }
-  s->d.sym = static_cast<uint8_t *>(s->b_sym.p);
-  s->d.off = static_cast<int64_t *>(s->b_off.p);
-  s->d.len = static_cast<int32_t *>(s->b_len.p);
-  s->d.n = n2;
+  SeqsetPtr s;
+  if (int const rc = seqset_alloc(c, std::move(h_len), std::move(h_off), total, std::move(h_nonacgt), s); rc != VSG_OK) { return rc; }
   if (n > 0) {
-    VSG_CUDA_OK(cudaMemcpyAsync(s->b_off.p, h_off.data(), sizeof(int64_t) * n2, cudaMemcpyHostToDevice, c->stream));
-    VSG_CUDA_OK(cudaMemcpyAsync(s->b_len.p, s->h_len.data(), sizeof(int32_t) * n2, cudaMemcpyHostToDevice, c->stream));
     int64_t const blocks = (n * 32 + 255) / 256;
     both_strands_kernel<<<static_cast<unsigned>(blocks), 256, 0, c->stream>>>(src->d, s->d.off, static_cast<uint8_t *>(s->b_sym.p));
     count_launch();
-    VSG_CUDA_OK(cudaStreamSynchronize(c->stream));  // h_off goes out of scope
+    VSG_CUDA_OK(cudaStreamSynchronize(c->stream));  // the kernel reads src, which the caller may release once this returns
   }
-  *out = guard.release();
+  out = std::move(s);
   return VSG_OK;
 }
 }  // namespace vsg
@@ -479,7 +461,10 @@ extern "C" int vsg_seqset_revcomp(vsg_ctx * c, const vsg_seqset * src, int64_t q
   if (q0 < 0 || n < 0 || q0 > src->d.n || n > src->d.n - q0) { Error::set("vsg_seqset_revcomp: range outside the sequence set"); return VSG_EINVAL; }
   if (src->device != c->device) { Error::set("vsg_seqset_revcomp: the sequence set lives on another device than the context"); return VSG_EINVAL; }
   VSG_CUDA_OK(cudaSetDevice(c->device));
-  return seqset_revcomp(c, src, q0, n, out);
+  SeqsetPtr s;
+  int const rc = seqset_revcomp(c, src, q0, n, s);
+  *out = s.release();
+  return rc;
 }
 
 extern "C" int64_t vsg_seqset_count(const vsg_seqset * s) { return s != nullptr ? s->d.n : 0; }
@@ -598,27 +583,344 @@ void launch_tb_ckpt_tasks(vsg_ctx * c, int R, bool general, const DevSeqs & qs, 
   else { launch_tb_ckpt_tasks_rt<16>(c, nthr, R, general, qs, ts, d_tasks, n, gate); }
 }
 
+template <int RT>
+void launch_tb_ckpt_pairs(vsg_ctx * c, const DevSeqs & qs, const DevSeqs & ts, const PairDesc * d_pairs, int np)
+{
+  cudaFuncSetAttribute(traceback_ckpt_pairs_kernel<RT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tb_ck_smem(RT)));
+  traceback_ckpt_pairs_kernel<RT><<<(np + TB_CK_THREADS - 1) / TB_CK_THREADS, TB_CK_THREADS, tb_ck_smem(RT), c->stream>>>(
+      c->sp2, qs, ts, d_pairs, np, static_cast<const uint2 *>(c->dir.p), static_cast<const uint2 *>(c->bnd.p),
+      static_cast<char *>(c->cigar_scratch.p), static_cast<int32_t *>(c->stats.p));
+  count_launch();
+}
+
+// The kernel class of a run of fast tasks: direction bits in one strip or in several strips, or checkpoints
+// (align_ckpt.cuh), stored or score-only (traceback on demand stores those of the few tasks it walks later, CK_RERUN).
+enum RunKind { RUN_DIR, RUN_DIR_STRIPS, RUN_CKPT, RUN_CKPT_SCOREONLY };
+constexpr int RUN_KINDS = RUN_CKPT_SCOREONLY + 1;
+
+struct ClassRun {  // a run of one kernel class in AlignPlan::fast
+  RunKind kind; int R; bool general; size_t first; int count;
+  // gated checkpoint runs: where the pair ids (2 * task + half) of [0] the leaders and ungated pairs, [1] the followers
+  // sit in AlignPlan::gate_ids
+  size_t ids_first[2]; int ids_count[2];
+  bool ckpt() const { return kind == RUN_CKPT || kind == RUN_CKPT_SCOREONLY; }
+};
+
 // A chunk = the tasks whose direction blocks share the scratch buffer at the same time.
-struct ClassRun { int R; bool general, multi, ckpt, scoreonly; size_t first; int count; };  // a run of one kernel class in all_fast
-struct ChunkPlan {
+struct Chunk {
   std::vector<ClassRun> runs;
   size_t exact_first = 0; int exact_count = 0;
   size_t pair_first = 0; int pair_count = 0;  // descriptors (CIGAR mode only)
   uint64_t dir_bytes = 0, bnd_elems = 0, he_elems = 0, cigar_bytes = 0;
-  int64_t cells = 0, nfast = 0, nexact = 0;
+  int64_t cells = 0, nfast = 0;
+  bool empty() const { return nfast == 0 && exact_count == 0; }
 };
 
-struct ChunkBuilder {  // the chunk being filled
-  // [general][0 = one strip, direction bits; 1 = several strips; 2 = checkpoints; 3 = checkpoints, score-only][rows per lane]
-  std::vector<FastTask> fast[2][4][FAST_RMAX + 1];
+// What an align call decides on the host before its first launch.
+struct AlignPlan {
+  struct HostPair { int64_t slot; int32_t st[VSG_STAT_WORDS]; };
+  std::vector<HostPair> host_pairs;   // pairs resolved without DP
+  std::vector<std::string> cigars;    // CIGAR mode: one per pair
+  std::vector<FastTask> fast;
   std::vector<ExactTask> exact;
-  uint64_t dir_bytes = 0, bnd_elems = 0, he_elems = 0, cigar_bytes = 0;
-  int64_t cells = 0, nfast = 0, nexact = 0;
-  int npairdesc = 0;
-  bool empty() const { return nfast == 0 && nexact == 0; }
+  std::vector<PairDesc> pairs;        // CIGAR mode only
+  std::vector<Chunk> chunks;
+  bool gated = false;                 // traceback on demand (TbGate): leader_of given, no CIGARs
+  std::vector<int> gate_ids;
+  int64_t n_stored = 0, n_scoreonly = 0;  // checkpoint tasks that store their checkpoints / run score-only
 };
 
 inline uint64_t align_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
+
+// Resolves the pairs the host can answer, groups the others by query into forward tasks (targets paired two by two)
+// and cuts the tasks into chunks that fit the direction-bit budget.  Makes no CUDA call.
+int plan_pairs(const vsg_ctx * c, const vsg_seqset * queries, const vsg_seqset * targets, int64_t npairs,
+               const uint32_t * qidx, const uint32_t * tidx, const int32_t * leader_of, bool want_cigar, AlignPlan & plan)
+{
+  ScoreParams const & sp = c->sp;
+  FastBound const fbound = fast_bound_of(sp);
+  FastBound const fbound2 = fast_bound_of(c->sp2);
+  // Small calls are latency-bound (the cluster driver's rounds, the tail rounds of a search).  For sequences of
+  // similar length one thread regenerating ~40 tiles takes a few hundred microseconds whatever the batch size while
+  // walking stored direction bits takes tens: below VSG_CKPT_MIN_PAIRS pairs (default 2048) such pairs use the
+  // direction-bit kernels.  A target several times longer than the query turns that around — the walk over stored
+  // bits pays one dependent HBM load per column of the end gap, the regenerated tiles cross it 32 columns at a time
+  // — so those pairs stay on the checkpoint kernels at any call size.  Both paths are bit-identical
+  // (tests/test_stress_gpu.py runs either).
+  const char * const ckpt_min_env = std::getenv("VSG_CKPT_MIN_PAIRS");   // read per call: tests switch it
+  int64_t const ckpt_min_pairs = ckpt_min_env != nullptr ? std::atoll(ckpt_min_env) : 2048LL;
+  bool const ckpt_any_size = c->ckpt_enabled && npairs >= ckpt_min_pairs;
+  // Traceback on demand (TbGate): a checkpoint task whose pairs are all group followers is usually never walked, so
+  // its forward pass stores no checkpoints (CK_SCOREONLY); the few that phase 2 does walk are recomputed with stores
+  // after phase 1 (CK_RERUN).  VSG_CK_SCOREONLY=0 stores the checkpoints of every task (A/B runs; same results).
+  const char * const so_env = std::getenv("VSG_CK_SCOREONLY");   // read per call: tests switch it
+  plan.gated = leader_of != nullptr && !want_cigar;
+  bool const scoreonly_ok = plan.gated && (so_env == nullptr || so_env[0] != '0');
+  if (want_cigar) { plan.cigars.resize(static_cast<size_t>(npairs)); }
+  if (plan.gated) { plan.gate_ids.reserve(static_cast<size_t>(npairs)); }
+  plan.fast.reserve(static_cast<size_t>(npairs) / 2 + 16);
+  Chunk cur;                                                   // the chunk being filled
+  std::vector<FastTask> cur_fast[2][RUN_KINDS][FAST_RMAX + 1];  // its fast tasks by [general][kind][rows per lane]
+  struct Cand { int64_t slot; uint32_t t; int32_t d; bool general; };
+  std::vector<Cand> group_fast;
+
+  auto host_pair = [&](int64_t slot) -> int32_t * {
+    plan.host_pairs.emplace_back();
+    plan.host_pairs.back().slot = slot;
+    std::memset(plan.host_pairs.back().st, 0, sizeof(int32_t) * VSG_STAT_WORDS);
+    return plan.host_pairs.back().st;
+  };
+
+  auto close_chunk = [&]() {
+    if (cur.empty()) { return; }
+    for (int g = 0; g < 2; g++) {
+      for (int kind = 0; kind < RUN_KINDS; kind++) {
+        for (int R = 1; R <= FAST_RMAX; R++) {
+          auto & v = cur_fast[g][kind][R];
+          if (v.empty()) { continue; }
+          // longest first: the tail of the grid is made of the short ones
+          auto const longer = [](const FastTask & a, const FastTask & b) { return a.dmax > b.dmax; };
+          if (!std::is_sorted(v.begin(), v.end(), longer)) { std::sort(v.begin(), v.end(), longer); }
+          ClassRun run{static_cast<RunKind>(kind), R, g != 0, plan.fast.size(), static_cast<int>(v.size()), {0, 0}, {0, 0}};
+          plan.fast.insert(plan.fast.end(), v.begin(), v.end());
+          v.clear();
+          if (run.ckpt()) { (run.kind == RUN_CKPT_SCOREONLY ? plan.n_scoreonly : plan.n_stored) += run.count; }
+          if (run.ckpt() && plan.gated) {
+            for (int pass = 0; pass < 2; pass++) {   // leaders and ungated pairs, then followers
+              run.ids_first[pass] = plan.gate_ids.size();
+              for (int k = 0; k < run.count; k++) {
+                FastTask const & ft = plan.fast[run.first + static_cast<size_t>(k)];
+                for (int half = 0; half < 2; half++) {
+                  int32_t const slot = half ? ft.out_hi : ft.out_lo;
+                  if (slot >= 0 && (leader_of[slot] >= 0) == (pass == 1)) { plan.gate_ids.push_back(2 * k + half); }
+                }
+              }
+              run.ids_count[pass] = static_cast<int>(plan.gate_ids.size() - run.ids_first[pass]);
+            }
+          }
+          cur.runs.push_back(run);
+        }
+      }
+    }
+    cur.exact_first = plan.exact.size() - static_cast<size_t>(cur.exact_count);
+    cur.pair_first = plan.pairs.size() - static_cast<size_t>(cur.pair_count);
+    plan.chunks.push_back(std::move(cur));
+    cur = Chunk{};
+  };
+
+  auto add_pairdesc = [&](uint32_t q, uint32_t t, int kind, int64_t slot, int R, int half, int dmax, uint64_t dir_off, uint64_t aux_off = 0) {
+    if (!want_cigar) { return; }
+    PairDesc pd{};
+    pd.q = q; pd.t = t; pd.dir_off = dir_off; pd.kind = kind; pd.out = static_cast<int32_t>(slot);
+    pd.R = R; pd.half = half; pd.dmax = dmax; pd.aux_off = aux_off;
+    pd.cigar_off = cur.cigar_bytes;
+    cur.cigar_bytes += static_cast<uint64_t>(queries->h_len[q]) + static_cast<uint64_t>(targets->h_len[t]) + 2;
+    plan.pairs.push_back(pd);
+    cur.pair_count++;
+  };
+
+  // resolve trivial pairs on the host, group by query, pair targets two by two
+  int64_t i = 0;
+  while (i < npairs) {
+    uint32_t const q = qidx[i];
+    if (q >= static_cast<uint64_t>(queries->d.n)) { Error::set("vsg_align_pairs: query index out of range"); return VSG_EINVAL; }
+    int64_t j = i;
+    while (j < npairs && qidx[j] == q) { j++; }
+    int const Q = queries->h_len[q];
+    bool const q_general = queries->h_nonacgt[q] != 0;
+    group_fast.clear();
+    for (int64_t k = i; k < j; k++) {
+      uint32_t const t = tidx[k];
+      if (t >= static_cast<uint64_t>(targets->d.n)) { Error::set("vsg_align_pairs: target index out of range"); return VSG_EINVAL; }
+      int const D = targets->h_len[t];
+      if (sp.fallback) { host_pair(k)[VSG_STAT_SCORE] = VSG_SCORE_SENTINEL; continue; }  // align_simd.cpp:1463-1479
+      if (Q == 0) {                                                                      // align_simd.cpp:1481-1539
+        int32_t * s = host_pair(k);
+        if (!fits16(0, D)) { s[VSG_STAT_SCORE] = VSG_SCORE_SENTINEL; continue; }
+        s[VSG_STAT_ALIGNED] = D; s[VSG_STAT_GAPS] = D;
+        if (D > 0) {
+          int64_t const a = -static_cast<int64_t>(sp.go[T_L]) - static_cast<int64_t>(D) * sp.ge[T_L];
+          int64_t const b = -static_cast<int64_t>(sp.go[T_R]) - static_cast<int64_t>(D) * sp.ge[T_R];
+          s[VSG_STAT_SCORE] = static_cast<int16_t>(std::max(a, b));
+          s[VSG_STAT_TRIM_LEFT] = -D; s[VSG_STAT_TRIM_RIGHT] = -D;
+          if (want_cigar) { plan.cigars[static_cast<size_t>(k)] = std::to_string(D) + "I"; }
+          s[VSG_STAT_CIGARLEN] = static_cast<int32_t>(std::to_string(D).size() + 1);
+        }
+        continue;
+      }
+      if (D == 0 || !fits16(Q, D)) { host_pair(k)[VSG_STAT_SCORE] = VSG_SCORE_SENTINEL; continue; }  // :1867-1882
+      bool const general = q_general || targets->h_nonacgt[t] != 0;
+      int R, ns;
+      fast_shape(Q, general, R, ns);
+      if (!c->fast_disabled && fast_path_ok(fbound, ns * 32 * R, D)) {
+        group_fast.push_back(Cand{k, t, D, general});
+      } else {
+        uint64_t const dirb = align_up(static_cast<uint64_t>(Q) * D, 16);
+        if (!cur.empty() && cur.dir_bytes + dirb > c->dir_budget) { close_chunk(); }
+        ExactTask et{};
+        et.q = q; et.t = t; et.out = static_cast<int32_t>(k);
+        et.dir_off = cur.dir_bytes; et.he_off = cur.he_elems;
+        add_pairdesc(q, t, PD_EXACT, k, 0, 0, 0, cur.dir_bytes);
+        cur.dir_bytes += dirb;
+        cur.he_elems += 2ULL * Q;
+        plan.exact.push_back(et);
+        cur.cells += static_cast<int64_t>(Q) * D; cur.exact_count++;
+      }
+    }
+    if (!group_fast.empty()) {
+      // similar lengths together (a warp runs for the longer of its two targets)
+      auto const by_len = [](const Cand & a, const Cand & b) {
+        if (a.general != b.general) { return a.general < b.general; }
+        if (a.d != b.d) { return a.d > b.d; }
+        return a.slot < b.slot;
+      };
+      if (!std::is_sorted(group_fast.begin(), group_fast.end(), by_len)) { std::sort(group_fast.begin(), group_fast.end(), by_len); }
+      size_t k = 0;
+      while (k < group_fast.size()) {
+        Cand const & a = group_fast[k];
+        bool const pair2 = (k + 1 < group_fast.size()) && (group_fast[k + 1].general == a.general);
+        Cand const & b = pair2 ? group_fast[k + 1] : a;
+        int R, ns;
+        fast_shape(Q, a.general, R, ns);
+        int const dmax = std::max(a.d, b.d);
+        // single-strip tasks go through the checkpoint kernel (no direction bits; align_ckpt.cuh) when its
+        // shifted scoring stays inside the exact range too
+        bool const ck = (ns == 1) && c->ckpt_enabled && (ckpt_any_size || dmax >= 3 * Q) && fast_path_ok(fbound2, 32 * R, dmax);
+        uint64_t const dirb = ck ? ckpt::row_elems(dmax) * sizeof(uint2) : static_cast<uint64_t>(ns) * fast_strip_bytes(dmax, R);
+        uint64_t const auxe = ck ? ckpt::col_elems(dmax, R) : (ns > 1 ? static_cast<uint64_t>(dmax) : 0);
+        if (!cur.empty() && cur.dir_bytes + dirb + (cur.bnd_elems + auxe) * sizeof(uint2) > c->dir_budget) { close_chunk(); }
+        FastTask ft{};
+        ft.q = q; ft.tlo = a.t; ft.thi = b.t;
+        ft.out_lo = static_cast<int32_t>(a.slot);
+        ft.out_hi = pair2 ? static_cast<int32_t>(b.slot) : -1;
+        ft.dmax = dmax;
+        ft.dir_off = ck ? cur.dir_bytes / sizeof(uint2) : cur.dir_bytes;   // checkpoints: uint2 element offsets
+        ft.bnd_off = cur.bnd_elems;
+        int const gbit = a.general ? 2 : 0;
+        int const pd_kind = ck ? PD_CKPT : PD_FAST;
+        add_pairdesc(q, a.t, pd_kind, a.slot, R, ck ? gbit : 0, dmax, ft.dir_off, ft.bnd_off);
+        if (pair2) { add_pairdesc(q, b.t, pd_kind, b.slot, R, ck ? (gbit | 1) : 1, dmax, ft.dir_off, ft.bnd_off); }
+        cur.dir_bytes += align_up(dirb, 32);
+        cur.bnd_elems += auxe;
+        bool const scoreonly = ck && scoreonly_ok && leader_of[a.slot] >= 0 && (!pair2 || leader_of[b.slot] >= 0);
+        RunKind const kind = scoreonly ? RUN_CKPT_SCOREONLY : (ck ? RUN_CKPT : (ns > 1 ? RUN_DIR_STRIPS : RUN_DIR));
+        cur_fast[a.general ? 1 : 0][kind][R].push_back(ft);
+        cur.cells += static_cast<int64_t>(Q) * a.d + (pair2 ? static_cast<int64_t>(Q) * b.d : 0);
+        cur.nfast += pair2 ? 2 : 1;
+        k += pair2 ? 2 : 1;
+      }
+    }
+    i = j;
+  }
+  close_chunk();
+  return VSG_OK;
+}
+
+// The CIGAR texts of one chunk after its forward pass: descriptors up, traceback with text (tb_done is recorded when it
+// ends), dense packing, texts home.
+int cigar_chunk(vsg_ctx * c, const DevSeqs & qs, const DevSeqs & ts, AlignPlan & plan, const Chunk & ch, cudaEvent_t tb_done)
+{
+  int const np = ch.pair_count;
+  int rc;
+  if ((rc = c->pairs.reserve(sizeof(PairDesc) * (static_cast<size_t>(np) + 1))) != VSG_OK) { return rc; }
+  if ((rc = c->cigar_scratch.reserve(ch.cigar_bytes + 64)) != VSG_OK) { return rc; }
+  if ((rc = c->cigar_dense.reserve(ch.cigar_bytes + 64)) != VSG_OK) { return rc; }
+  if ((rc = c->cigar_len.reserve(sizeof(int64_t) * (static_cast<size_t>(np) + 1))) != VSG_OK) { return rc; }
+  if ((rc = c->cigar_offs.reserve(sizeof(int64_t) * (static_cast<size_t>(np) + 1))) != VSG_OK) { return rc; }
+  PairDesc const * hpairs = plan.pairs.data() + ch.pair_first;
+  PairDesc * d_pairs = static_cast<PairDesc *>(c->pairs.p);
+  int32_t * const d_stats = static_cast<int32_t *>(c->stats.p);
+  VSG_CUDA_OK(cudaMemcpyAsync(d_pairs, hpairs, sizeof(PairDesc) * np, cudaMemcpyHostToDevice, c->stream));
+  traceback_kernel<true><<<(np + 127) / 128, 128, 0, c->stream>>>(c->sp, qs, ts, d_pairs, np, static_cast<uint8_t *>(c->dir.p),
+                                                                  static_cast<char *>(c->cigar_scratch.p), d_stats);
+  count_launch();
+  bool ck8 = false, ck16 = false;
+  for (auto const & run : ch.runs) { if (run.ckpt()) { (run.R <= 8 ? ck8 : ck16) = true; } }
+  if (ck8) { launch_tb_ckpt_pairs<8>(c, qs, ts, d_pairs, np); }
+  if (ck16) { launch_tb_ckpt_pairs<16>(c, qs, ts, d_pairs, np); }
+  VSG_CUDA_OK(cudaEventRecord(tb_done, c->stream));
+  cigar_len_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(d_pairs, d_stats, np, static_cast<int64_t *>(c->cigar_len.p));
+  count_launch();
+  size_t tmp_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, static_cast<int64_t *>(c->cigar_len.p),
+                                static_cast<int64_t *>(c->cigar_offs.p), np, c->stream);
+  if ((rc = c->cub_tmp.reserve(tmp_bytes + 16)) != VSG_OK) { return rc; }
+  cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tmp_bytes, static_cast<int64_t *>(c->cigar_len.p),
+                                static_cast<int64_t *>(c->cigar_offs.p), np, c->stream);
+  count_launch();
+  cigar_gather_kernel<<<np, 64, 0, c->stream>>>(d_pairs, np, qs, ts, d_stats, static_cast<int64_t *>(c->cigar_offs.p),
+                                                static_cast<char *>(c->cigar_scratch.p), static_cast<char *>(c->cigar_dense.p));
+  count_launch();
+  std::vector<int64_t> h_offs(static_cast<size_t>(np)), h_lens(static_cast<size_t>(np));
+  VSG_CUDA_OK(cudaMemcpyAsync(h_offs.data(), c->cigar_offs.p, sizeof(int64_t) * np, cudaMemcpyDeviceToHost, c->stream));
+  VSG_CUDA_OK(cudaMemcpyAsync(h_lens.data(), c->cigar_len.p, sizeof(int64_t) * np, cudaMemcpyDeviceToHost, c->stream));
+  VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
+  int64_t const total = np > 0 ? h_offs[static_cast<size_t>(np) - 1] + h_lens[static_cast<size_t>(np) - 1] : 0;
+  std::vector<char> dense(static_cast<size_t>(total) + 1);
+  if (total > 0) {
+    VSG_CUDA_OK(cudaMemcpyAsync(dense.data(), c->cigar_dense.p, static_cast<size_t>(total), cudaMemcpyDeviceToHost, c->stream));
+    VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
+  }
+  for (int p = 0; p < np; p++) { plan.cigars[static_cast<size_t>(hpairs[p].out)] = std::string(dense.data() + h_offs[static_cast<size_t>(p)]); }
+  return VSG_OK;
+}
+
+// Chunk ci of the plan: the forward pass, then the statistics traceback or the CIGAR pipeline, timed by the chunk's three
+// events.  A gated call walks each checkpoint run in two phases: its leaders and ungated pairs first, then (once the
+// CK_RERUN pass has stored the checkpoints of the score-only tasks phase 2 will walk) its followers.  `gate` holds the
+// device gate ids, leader_of and the identity test of a gated call, and gates nothing otherwise.
+int launch_chunk(vsg_ctx * c, const DevSeqs & qs, const DevSeqs & ts, AlignPlan & plan, size_t ci, bool want_cigar,
+                 const TbGate & gate, int * d_rerun)
+{
+  Chunk const & ch = plan.chunks[ci];
+  cudaEvent_t const * const ev = c->ev_pool.data() + 3 * ci;
+  FastTask const * const d_fast = static_cast<const FastTask *>(c->tasks_fast.p);
+  ExactTask const * const d_exact = static_cast<const ExactTask *>(c->tasks_exact.p);
+  uint8_t * const d_dir = static_cast<uint8_t *>(c->dir.p);
+  int32_t * const d_stats = static_cast<int32_t *>(c->stats.p);
+  VSG_CUDA_OK(cudaEventRecord(ev[0], c->stream));
+  for (auto const & run : ch.runs) {
+    switch (run.kind) {
+      case RUN_DIR: launch_fast(c, run.R, run.general, false, qs, ts, d_fast + run.first, run.count); break;
+      case RUN_DIR_STRIPS: launch_fast(c, run.R, run.general, true, qs, ts, d_fast + run.first, run.count); break;
+      case RUN_CKPT: launch_ckpt(c, run.R, run.general, CK_STORE, qs, ts, d_fast + run.first, run.count); break;
+      case RUN_CKPT_SCOREONLY: launch_ckpt(c, run.R, run.general, CK_SCOREONLY, qs, ts, d_fast + run.first, run.count); break;
+    }
+  }
+  if (ch.exact_count > 0) {
+    nw_exact_kernel<<<(ch.exact_count + 63) / 64, 64, 0, c->stream>>>(c->sp, qs, ts, d_exact + ch.exact_first, ch.exact_count,
+                                                                      d_dir, static_cast<int16_t *>(c->he.p), d_stats);
+    count_launch();
+  }
+  VSG_CUDA_OK(cudaEventRecord(ev[1], c->stream));
+  if (want_cigar) { return cigar_chunk(c, qs, ts, plan, ch, ev[2]); }
+  auto const walk_ckpt = [&](const ClassRun & run, int phase) {   // phase 1: leaders and ungated pairs, 2: followers
+    TbGate g = gate;
+    if (plan.gated) { g.ids += run.ids_first[phase - 1]; g.nids = run.ids_count[phase - 1]; g.phase = phase; }
+    launch_tb_ckpt_tasks(c, run.R, run.general, qs, ts, d_fast + run.first, run.count, g);
+  };
+  if (plan.gated) {
+    // phase 1 of every checkpoint run: the leaders' verdicts must be in before any follower looks
+    for (auto const & run : ch.runs) { if (run.ckpt()) { walk_ckpt(run, 1); } }
+    // the checkpoints of the score-only tasks phase 2 will walk (a follower whose leader was not accepted)
+    for (auto const & run : ch.runs) {
+      if (run.kind == RUN_CKPT_SCOREONLY) { launch_ckpt(c, run.R, run.general, CK_RERUN, qs, ts, d_fast + run.first, run.count, gate.leader_of, d_rerun); }
+    }
+  }
+  for (auto const & run : ch.runs) {
+    if (run.ckpt()) { walk_ckpt(run, 2); continue; }
+    traceback_fast_tasks_kernel<<<(2 * run.count + 127) / 128, 128, 0, c->stream>>>(c->sp, qs, ts, d_fast + run.first, run.count,
+                                                                                    run.R, d_dir, d_stats);
+    count_launch();
+  }
+  if (ch.exact_count > 0) {
+    traceback_exact_tasks_kernel<<<(ch.exact_count + 127) / 128, 128, 0, c->stream>>>(c->sp, qs, ts, d_exact + ch.exact_first,
+                                                                                     ch.exact_count, d_dir, d_stats);
+    count_launch();
+  }
+  VSG_CUDA_OK(cudaEventRecord(ev[2], c->stream));
+  return VSG_OK;
+}
 
 }  // namespace
 
@@ -683,397 +985,84 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
   if ((rc = c->h_stats.reserve(sizeof(int32_t) * VSG_STAT_WORDS * static_cast<size_t>(npairs))) != VSG_OK) { return rc; }
   if ((rc = c->stats.reserve(sizeof(int32_t) * VSG_STAT_WORDS * static_cast<size_t>(npairs) + 64)) != VSG_OK) { return rc; }
   int32_t * const hs = static_cast<int32_t *>(c->h_stats.p);
-  struct HostPair { int64_t slot; int32_t st[VSG_STAT_WORDS]; };
-  std::vector<HostPair> host_pairs;
-  std::vector<std::string> cigars;
-  if (want_cigar) { cigars.resize(static_cast<size_t>(npairs)); }
-
-  ScoreParams const & sp = c->sp;
-  FastBound const fbound = fast_bound_of(sp);
-  FastBound const fbound2 = fast_bound_of(c->sp2);
-  // Small calls are latency-bound (the cluster driver's rounds, the tail rounds of a search).  For sequences of
-  // similar length one thread regenerating ~40 tiles takes a few hundred microseconds whatever the batch size while
-  // walking stored direction bits takes tens: below VSG_CKPT_MIN_PAIRS pairs (default 2048) such pairs use the
-  // direction-bit kernels.  A target several times longer than the query turns that around — the walk over stored
-  // bits pays one dependent HBM load per column of the end gap, the regenerated tiles cross it 32 columns at a time
-  // — so those pairs stay on the checkpoint kernels at any call size.  Both paths are bit-identical
-  // (tests/test_stress_gpu.py runs either).
-  const char * const ckpt_min_env = std::getenv("VSG_CKPT_MIN_PAIRS");   // read per call: tests switch it
-  int64_t const ckpt_min_pairs = ckpt_min_env != nullptr ? std::atoll(ckpt_min_env) : 2048LL;
-  bool const ckpt_any_size = c->ckpt_enabled && npairs >= ckpt_min_pairs;
-  // Traceback on demand (TbGate): a checkpoint task whose pairs are all group followers is usually never walked, so
-  // its forward pass stores no checkpoints (CK_SCOREONLY); the few that phase 2 does walk are recomputed with stores
-  // after phase 1 (CK_RERUN).  VSG_CK_SCOREONLY=0 stores the checkpoints of every task (A/B runs; same results).
-  const char * const so_env = std::getenv("VSG_CK_SCOREONLY");   // read per call: tests switch it
-  bool const scoreonly_ok = leader_of != nullptr && !want_cigar && (so_env == nullptr || so_env[0] != '0');
-  std::vector<FastTask> all_fast;
-  std::vector<ExactTask> all_exact;
-  std::vector<PairDesc> all_pairs;  // CIGAR mode only
-  std::vector<ChunkPlan> plans;
-  ChunkBuilder cb;
-  all_fast.reserve(static_cast<size_t>(npairs) / 2 + 16);
-  struct Cand { int64_t slot; uint32_t t; int32_t d; bool general; };
-  std::vector<Cand> group_fast;
-
-  auto host_pair = [&](int64_t slot) -> int32_t * {
-    host_pairs.emplace_back();
-    host_pairs.back().slot = slot;
-    std::memset(host_pairs.back().st, 0, sizeof(int32_t) * VSG_STAT_WORDS);
-    return host_pairs.back().st;
-  };
-
-  auto close_chunk = [&]() {
-    if (cb.empty()) { return; }
-    ChunkPlan pl;
-    for (int gm = 0; gm < 8; gm++) {
-      int const g = gm / 4, m = gm % 4;
-      for (int R = 1; R <= FAST_RMAX; R++) {
-        auto & v = cb.fast[g][m][R];
-        if (v.empty()) { continue; }
-        // longest first: the tail of the grid is made of the short ones
-        auto const longer = [](const FastTask & a, const FastTask & b) { return a.dmax > b.dmax; };
-        if (!std::is_sorted(v.begin(), v.end(), longer)) { std::sort(v.begin(), v.end(), longer); }
-        pl.runs.push_back(ClassRun{R, g != 0, m == 1, m >= 2, m == 3, all_fast.size(), static_cast<int>(v.size())});
-        all_fast.insert(all_fast.end(), v.begin(), v.end());
-        v.clear();
-      }
-    }
-    pl.exact_first = all_exact.size(); pl.exact_count = static_cast<int>(cb.exact.size());
-    all_exact.insert(all_exact.end(), cb.exact.begin(), cb.exact.end());
-    cb.exact.clear();
-    pl.pair_first = all_pairs.size() - static_cast<size_t>(cb.npairdesc); pl.pair_count = cb.npairdesc;
-    pl.dir_bytes = cb.dir_bytes; pl.bnd_elems = cb.bnd_elems; pl.he_elems = cb.he_elems; pl.cigar_bytes = cb.cigar_bytes;
-    pl.cells = cb.cells; pl.nfast = cb.nfast; pl.nexact = cb.nexact;
-    plans.push_back(std::move(pl));
-    cb.dir_bytes = cb.bnd_elems = cb.he_elems = cb.cigar_bytes = 0;
-    cb.cells = cb.nfast = cb.nexact = 0; cb.npairdesc = 0;
-  };
-
-  auto add_pairdesc = [&](uint32_t q, uint32_t t, int kind, int64_t slot, int R, int half, int dmax, uint64_t dir_off, uint64_t aux_off = 0) {
-    if (!want_cigar) { return; }
-    PairDesc pd{};
-    pd.q = q; pd.t = t; pd.dir_off = dir_off; pd.kind = kind; pd.out = static_cast<int32_t>(slot);
-    pd.R = R; pd.half = half; pd.dmax = dmax; pd.aux_off = aux_off;
-    pd.cigar_off = cb.cigar_bytes;
-    cb.cigar_bytes += static_cast<uint64_t>(queries->h_len[q]) + static_cast<uint64_t>(targets->h_len[t]) + 2;
-    all_pairs.push_back(pd);
-    cb.npairdesc++;
-  };
-
-  // ---- plan: resolve trivial pairs on the host, group by query, pair targets two by two ----------
-  int64_t i = 0;
-  while (i < npairs) {
-    uint32_t const q = qidx[i];
-    if (q >= static_cast<uint64_t>(queries->d.n)) { Error::set("vsg_align_pairs: query index out of range"); return VSG_EINVAL; }
-    int64_t j = i;
-    while (j < npairs && qidx[j] == q) { j++; }
-    int const Q = queries->h_len[q];
-    bool const q_general = queries->h_nonacgt[q] != 0;
-    group_fast.clear();
-    for (int64_t k = i; k < j; k++) {
-      uint32_t const t = tidx[k];
-      if (t >= static_cast<uint64_t>(targets->d.n)) { Error::set("vsg_align_pairs: target index out of range"); return VSG_EINVAL; }
-      int const D = targets->h_len[t];
-      if (sp.fallback) { host_pair(k)[VSG_STAT_SCORE] = VSG_SCORE_SENTINEL; continue; }  // align_simd.cpp:1463-1479
-      if (Q == 0) {                                                                      // align_simd.cpp:1481-1539
-        int32_t * s = host_pair(k);
-        if (!fits16(0, D)) { s[VSG_STAT_SCORE] = VSG_SCORE_SENTINEL; continue; }
-        s[VSG_STAT_ALIGNED] = D; s[VSG_STAT_GAPS] = D;
-        if (D > 0) {
-          int64_t const a = -static_cast<int64_t>(sp.go[T_L]) - static_cast<int64_t>(D) * sp.ge[T_L];
-          int64_t const b = -static_cast<int64_t>(sp.go[T_R]) - static_cast<int64_t>(D) * sp.ge[T_R];
-          s[VSG_STAT_SCORE] = static_cast<int16_t>(std::max(a, b));
-          s[VSG_STAT_TRIM_LEFT] = -D; s[VSG_STAT_TRIM_RIGHT] = -D;
-          if (want_cigar) { cigars[static_cast<size_t>(k)] = std::to_string(D) + "I"; }
-          s[VSG_STAT_CIGARLEN] = static_cast<int32_t>(std::to_string(D).size() + 1);
-        }
-        continue;
-      }
-      if (D == 0 || !fits16(Q, D)) { host_pair(k)[VSG_STAT_SCORE] = VSG_SCORE_SENTINEL; continue; }  // :1867-1882
-      bool const general = q_general || targets->h_nonacgt[t] != 0;
-      int R, ns;
-      fast_shape(Q, general, R, ns);
-      if (!c->fast_disabled && fast_path_ok(fbound, ns * 32 * R, D)) {
-        group_fast.push_back(Cand{k, t, D, general});
-      } else {
-        uint64_t const dirb = align_up(static_cast<uint64_t>(Q) * D, 16);
-        if (!cb.empty() && cb.dir_bytes + dirb > c->dir_budget) { close_chunk(); }
-        ExactTask et{};
-        et.q = q; et.t = t; et.out = static_cast<int32_t>(k);
-        et.dir_off = cb.dir_bytes; et.he_off = cb.he_elems;
-        add_pairdesc(q, t, 1, k, 0, 0, 0, cb.dir_bytes);
-        cb.dir_bytes += dirb;
-        cb.he_elems += 2ULL * Q;
-        cb.exact.push_back(et);
-        cb.cells += static_cast<int64_t>(Q) * D; cb.nexact++;
-      }
-    }
-    if (!group_fast.empty()) {
-      // similar lengths together (a warp runs for the longer of its two targets)
-      auto const by_len = [](const Cand & a, const Cand & b) {
-        if (a.general != b.general) { return a.general < b.general; }
-        if (a.d != b.d) { return a.d > b.d; }
-        return a.slot < b.slot;
-      };
-      if (!std::is_sorted(group_fast.begin(), group_fast.end(), by_len)) { std::sort(group_fast.begin(), group_fast.end(), by_len); }
-      size_t k = 0;
-      while (k < group_fast.size()) {
-        Cand const & a = group_fast[k];
-        bool const pair2 = (k + 1 < group_fast.size()) && (group_fast[k + 1].general == a.general);
-        Cand const & b = pair2 ? group_fast[k + 1] : a;
-        int R, ns;
-        fast_shape(Q, a.general, R, ns);
-        int const dmax = std::max(a.d, b.d);
-        // single-strip tasks go through the checkpoint kernel (no direction bits; align_ckpt.cuh) when its
-        // shifted scoring stays inside the exact range too
-        bool const ck = (ns == 1) && c->ckpt_enabled && (ckpt_any_size || dmax >= 3 * Q) && fast_path_ok(fbound2, 32 * R, dmax);
-        uint64_t const dirb = ck ? ckpt::row_elems(dmax) * sizeof(uint2) : static_cast<uint64_t>(ns) * fast_strip_bytes(dmax, R);
-        uint64_t const auxe = ck ? ckpt::col_elems(dmax, R) : (ns > 1 ? static_cast<uint64_t>(dmax) : 0);
-        if (!cb.empty() && cb.dir_bytes + dirb + (cb.bnd_elems + auxe) * sizeof(uint2) > c->dir_budget) { close_chunk(); }
-        FastTask ft{};
-        ft.q = q; ft.tlo = a.t; ft.thi = b.t;
-        ft.out_lo = static_cast<int32_t>(a.slot);
-        ft.out_hi = pair2 ? static_cast<int32_t>(b.slot) : -1;
-        ft.dmax = dmax;
-        ft.dir_off = ck ? cb.dir_bytes / sizeof(uint2) : cb.dir_bytes;   // checkpoints: uint2 element offsets
-        ft.bnd_off = cb.bnd_elems;
-        int const gbit = a.general ? 2 : 0;
-        add_pairdesc(q, a.t, ck ? 2 : 0, a.slot, R, ck ? gbit : 0, dmax, ft.dir_off, ft.bnd_off);
-        if (pair2) { add_pairdesc(q, b.t, ck ? 2 : 0, b.slot, R, ck ? (gbit | 1) : 1, dmax, ft.dir_off, ft.bnd_off); }
-        cb.dir_bytes += align_up(dirb, 32);
-        cb.bnd_elems += auxe;
-        bool const scoreonly = ck && scoreonly_ok && leader_of[a.slot] >= 0 && (!pair2 || leader_of[b.slot] >= 0);
-        cb.fast[a.general ? 1 : 0][scoreonly ? 3 : (ck ? 2 : (ns > 1 ? 1 : 0))][R].push_back(ft);
-        cb.cells += static_cast<int64_t>(Q) * a.d + (pair2 ? static_cast<int64_t>(Q) * b.d : 0);
-        cb.nfast += pair2 ? 2 : 1;
-        k += pair2 ? 2 : 1;
-      }
-    }
-    i = j;
-  }
-  close_chunk();
+  AlignPlan plan;
+  if ((rc = plan_pairs(c, queries, targets, npairs, qidx, tidx, leader_of, want_cigar, plan)) != VSG_OK) { return rc; }
   auto const t_planned = std::chrono::steady_clock::now();
 
-  // ---- upload every task of the call once; size the scratch for the largest chunk ----------------
-  uint64_t max_dir = 0, max_bnd = 0, max_he = 0, max_cig = 0;
-  for (auto const & pl : plans) {
-    max_dir = std::max(max_dir, pl.dir_bytes); max_bnd = std::max(max_bnd, pl.bnd_elems);
-    max_he = std::max(max_he, pl.he_elems); max_cig = std::max(max_cig, pl.cigar_bytes);
-  }
-  if (!plans.empty()) {
+  // ---- launch: every task of the call uploaded once, the scratch sized for the largest chunk, then chunk by chunk --
+  TbGate gate{nullptr, 0, nullptr, 0, 2, 0.0};   // ungated: every pair of the tasks
+  if (!plan.chunks.empty()) {
+    uint64_t max_dir = 0, max_bnd = 0, max_he = 0;
+    for (auto const & ch : plan.chunks) {
+      max_dir = std::max(max_dir, ch.dir_bytes); max_bnd = std::max(max_bnd, ch.bnd_elems); max_he = std::max(max_he, ch.he_elems);
+    }
     if ((rc = c->dir.reserve(max_dir + 256)) != VSG_OK) { return rc; }
     if ((rc = c->bnd.reserve(sizeof(uint2) * (max_bnd + 1))) != VSG_OK) { return rc; }
     if ((rc = c->he.reserve(sizeof(int16_t) * (max_he + 1))) != VSG_OK) { return rc; }
-    if ((rc = c->tasks_fast.reserve(sizeof(FastTask) * (all_fast.size() + 1))) != VSG_OK) { return rc; }
-    if ((rc = c->tasks_exact.reserve(sizeof(ExactTask) * (all_exact.size() + 1))) != VSG_OK) { return rc; }
-    size_t const fb = sizeof(FastTask) * all_fast.size(), eb = sizeof(ExactTask) * all_exact.size();
+    if ((rc = c->tasks_fast.reserve(sizeof(FastTask) * (plan.fast.size() + 1))) != VSG_OK) { return rc; }
+    if ((rc = c->tasks_exact.reserve(sizeof(ExactTask) * (plan.exact.size() + 1))) != VSG_OK) { return rc; }
+    size_t const fb = sizeof(FastTask) * plan.fast.size(), eb = sizeof(ExactTask) * plan.exact.size();
     if ((rc = c->h_tasks.reserve(fb + eb + 64)) != VSG_OK) { return rc; }
     char * hp = static_cast<char *>(c->h_tasks.p);
     if (fb > 0) {
-      std::memcpy(hp, all_fast.data(), fb);
+      std::memcpy(hp, plan.fast.data(), fb);
       VSG_CUDA_OK(cudaMemcpyAsync(c->tasks_fast.p, hp, fb, cudaMemcpyHostToDevice, c->stream));
     }
     if (eb > 0) {
-      std::memcpy(hp + fb, all_exact.data(), eb);
+      std::memcpy(hp + fb, plan.exact.data(), eb);
       VSG_CUDA_OK(cudaMemcpyAsync(c->tasks_exact.p, hp + fb, eb, cudaMemcpyHostToDevice, c->stream));
     }
-  }
-  // traceback on demand: per checkpoint run, the pair ids of the leaders (and ungated pairs) and of the followers
-  bool const gated = leader_of != nullptr && !want_cigar && !plans.empty();
-  struct GateRun { size_t lead_first, lead_count, foll_first, foll_count; };
-  std::vector<std::vector<GateRun>> gate_runs;
-  int const * d_gate_ids = nullptr;
-  int32_t const * d_leader = nullptr;
-  if (gated) {
-    std::vector<int> ids;
-    ids.reserve(static_cast<size_t>(npairs));
-    gate_runs.resize(plans.size());
-    for (size_t ci = 0; ci < plans.size(); ci++) {
-      for (auto const & run : plans[ci].runs) {
-        GateRun g{ids.size(), 0, 0, 0};
-        if (run.ckpt) {
-          for (int pass = 0; pass < 2; pass++) {
-            if (pass == 1) { g.lead_count = ids.size() - g.lead_first; g.foll_first = ids.size(); }
-            for (int k = 0; k < run.count; k++) {
-              FastTask const & ft = all_fast[run.first + static_cast<size_t>(k)];
-              for (int half = 0; half < 2; half++) {
-                int32_t const slot = half ? ft.out_hi : ft.out_lo;
-                if (slot < 0) { continue; }
-                bool const follower = leader_of[slot] >= 0;
-                if (follower == (pass == 1)) { ids.push_back(2 * k + half); }
-              }
-            }
-          }
-          g.foll_count = ids.size() - g.foll_first;
-        }
-        gate_runs[ci].push_back(g);
-      }
+    if (plan.gated) {   // traceback on demand: the gate ids of every checkpoint run, then leader_of
+      size_t const nids = plan.gate_ids.size();
+      if ((rc = c->gate.reserve(sizeof(int) * (nids + static_cast<size_t>(npairs)) + 64)) != VSG_OK) { return rc; }
+      int * const dg = static_cast<int *>(c->gate.p);
+      // pageable sources: both copies are staged before cudaMemcpyAsync returns
+      if (nids > 0) { VSG_CUDA_OK(cudaMemcpyAsync(dg, plan.gate_ids.data(), sizeof(int) * nids, cudaMemcpyHostToDevice, c->stream)); }
+      VSG_CUDA_OK(cudaMemcpyAsync(dg + nids, leader_of, sizeof(int32_t) * static_cast<size_t>(npairs), cudaMemcpyHostToDevice, c->stream));
+      gate = TbGate{dg, 0, dg + nids, 0, gate_iddef, gate_threshold};
+      // "not computed" everywhere until a kernel says otherwise
+      VSG_CUDA_OK(cudaMemsetAsync(c->stats.p, 0xff, sizeof(int32_t) * VSG_STAT_WORDS * static_cast<size_t>(npairs), c->stream));
     }
-    if ((rc = c->gate.reserve(sizeof(int) * (ids.size() + static_cast<size_t>(npairs)) + 64)) != VSG_OK) { return rc; }
-    int * const dg = static_cast<int *>(c->gate.p);
-    // pageable sources: both copies are staged before cudaMemcpyAsync returns
-    if (!ids.empty()) { VSG_CUDA_OK(cudaMemcpyAsync(dg, ids.data(), sizeof(int) * ids.size(), cudaMemcpyHostToDevice, c->stream)); }
-    VSG_CUDA_OK(cudaMemcpyAsync(dg + ids.size(), leader_of, sizeof(int32_t) * static_cast<size_t>(npairs), cudaMemcpyHostToDevice, c->stream));
-    d_gate_ids = dg;
-    d_leader = dg + ids.size();
-    // "not computed" everywhere until a kernel says otherwise
-    VSG_CUDA_OK(cudaMemsetAsync(c->stats.p, 0xff, sizeof(int32_t) * VSG_STAT_WORDS * static_cast<size_t>(npairs), c->stream));
   }
   // events: 3 per chunk
-  while (c->ev_pool.size() < 3 * plans.size()) {
+  while (c->ev_pool.size() < 3 * plan.chunks.size()) {
     cudaEvent_t e;
     VSG_CUDA_OK(cudaEventCreate(&e));
     c->ev_pool.push_back(e);
   }
-
-  // VSG_TRACE and ck_counts: how many checkpoint tasks stored their checkpoints, ran score-only, and were re-run with stores
-  int64_t n_stored = 0, n_scoreonly = 0;
+  // VSG_TRACE and ck_counts: how many score-only checkpoint tasks were re-run with stores
   int * d_rerun = nullptr;
-  if (trace || ck_counts != nullptr) {
-    for (auto const & pl : plans) {
-      for (auto const & run : pl.runs) { if (run.ckpt) { (run.scoreonly ? n_scoreonly : n_stored) += run.count; } }
-    }
-    if (n_scoreonly > 0) {
-      if ((rc = c->rerun_count.reserve(64)) != VSG_OK) { return rc; }
-      d_rerun = static_cast<int *>(c->rerun_count.p);
-      VSG_CUDA_OK(cudaMemsetAsync(d_rerun, 0, sizeof(int), c->stream));
-    }
+  if ((trace || ck_counts != nullptr) && plan.n_scoreonly > 0) {
+    if ((rc = c->rerun_count.reserve(64)) != VSG_OK) { return rc; }
+    d_rerun = static_cast<int *>(c->rerun_count.p);
+    VSG_CUDA_OK(cudaMemsetAsync(d_rerun, 0, sizeof(int), c->stream));
   }
-  FastTask * const d_fast = static_cast<FastTask *>(c->tasks_fast.p);
-  ExactTask * const d_exact = static_cast<ExactTask *>(c->tasks_exact.p);
-  int32_t * const d_stats = static_cast<int32_t *>(c->stats.p);
-  uint8_t * const d_dir = static_cast<uint8_t *>(c->dir.p);
+  for (size_t ci = 0; ci < plan.chunks.size(); ci++) {
+    if ((rc = launch_chunk(c, queries->d, targets->d, plan, ci, want_cigar, gate, d_rerun)) != VSG_OK) { return rc; }
+  }
 
-  for (size_t ci = 0; ci < plans.size(); ci++) {
-    ChunkPlan const & pl = plans[ci];
-    VSG_CUDA_OK(cudaEventRecord(c->ev_pool[3 * ci], c->stream));
-    for (auto const & run : pl.runs) {
-      if (run.ckpt) { launch_ckpt(c, run.R, run.general, run.scoreonly ? CK_SCOREONLY : CK_STORE, queries->d, targets->d, d_fast + run.first, run.count); }
-      else { launch_fast(c, run.R, run.general, run.multi, queries->d, targets->d, d_fast + run.first, run.count); }
-    }
-    if (pl.exact_count > 0) {
-      nw_exact_kernel<<<(pl.exact_count + 63) / 64, 64, 0, c->stream>>>(sp, queries->d, targets->d, d_exact + pl.exact_first,
-                                                                        pl.exact_count, d_dir, static_cast<int16_t *>(c->he.p), d_stats);
-      count_launch();
-    }
-    VSG_CUDA_OK(cudaEventRecord(c->ev_pool[3 * ci + 1], c->stream));
-    if (!want_cigar) {
-      TbGate const no_gate{nullptr, 0, nullptr, 0, 2, 0.0};
-      if (gated) {
-        // phase 1: leaders and ungated pairs of every checkpoint run (their verdicts must be in before any follower looks)
-        for (size_t ri = 0; ri < pl.runs.size(); ri++) {
-          auto const & run = pl.runs[ri];
-          if (!run.ckpt) { continue; }
-          GateRun const & g = gate_runs[ci][ri];
-          TbGate const g1{d_gate_ids + g.lead_first, static_cast<int>(g.lead_count), d_leader, 1, gate_iddef, gate_threshold};
-          launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, g1);
-        }
-        // the checkpoints of the score-only tasks phase 2 will walk (a follower whose leader was not accepted)
-        for (auto const & run : pl.runs) {
-          if (run.scoreonly) {
-            launch_ckpt(c, run.R, run.general, CK_RERUN, queries->d, targets->d, d_fast + run.first, run.count, d_leader, d_rerun);
-          }
-        }
-      }
-      for (size_t ri = 0; ri < pl.runs.size(); ri++) {
-        auto const & run = pl.runs[ri];
-        if (run.ckpt) {
-          if (gated) {
-            GateRun const & g = gate_runs[ci][ri];
-            TbGate const g2{d_gate_ids + g.foll_first, static_cast<int>(g.foll_count), d_leader, 2, gate_iddef, gate_threshold};
-            launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, g2);
-            continue;
-          }
-          launch_tb_ckpt_tasks(c, run.R, run.general, queries->d, targets->d, d_fast + run.first, run.count, no_gate);
-          continue;
-        }
-        int const nthr = 2 * run.count;
-        traceback_fast_tasks_kernel<<<(nthr + 127) / 128, 128, 0, c->stream>>>(sp, queries->d, targets->d, d_fast + run.first,
-                                                                               run.count, run.R, d_dir, d_stats);
-        count_launch();
-      }
-      if (pl.exact_count > 0) {
-        traceback_exact_tasks_kernel<<<(pl.exact_count + 127) / 128, 128, 0, c->stream>>>(sp, queries->d, targets->d,
-                                                                                         d_exact + pl.exact_first, pl.exact_count, d_dir, d_stats);
-        count_launch();
-      }
-      VSG_CUDA_OK(cudaEventRecord(c->ev_pool[3 * ci + 2], c->stream));
-    } else {
-      // CIGAR texts: descriptors up, traceback with text, dense packing, texts home — per chunk
-      int const np = pl.pair_count;
-      if ((rc = c->pairs.reserve(sizeof(PairDesc) * (static_cast<size_t>(np) + 1))) != VSG_OK) { return rc; }
-      if ((rc = c->cigar_scratch.reserve(pl.cigar_bytes + 64)) != VSG_OK) { return rc; }
-      if ((rc = c->cigar_dense.reserve(pl.cigar_bytes + 64)) != VSG_OK) { return rc; }
-      if ((rc = c->cigar_len.reserve(sizeof(int64_t) * (static_cast<size_t>(np) + 1))) != VSG_OK) { return rc; }
-      if ((rc = c->cigar_offs.reserve(sizeof(int64_t) * (static_cast<size_t>(np) + 1))) != VSG_OK) { return rc; }
-      PairDesc const * hpairs = all_pairs.data() + pl.pair_first;
-      PairDesc * d_pairs = static_cast<PairDesc *>(c->pairs.p);
-      VSG_CUDA_OK(cudaMemcpyAsync(d_pairs, hpairs, sizeof(PairDesc) * np, cudaMemcpyHostToDevice, c->stream));
-      traceback_kernel<true><<<(np + 127) / 128, 128, 0, c->stream>>>(sp, queries->d, targets->d, d_pairs, np, d_dir,
-                                                                      static_cast<char *>(c->cigar_scratch.p), d_stats);
-      count_launch();
-      bool ck8 = false, ck16 = false;
-      for (auto const & run : pl.runs) { if (run.ckpt) { (run.R <= 8 ? ck8 : ck16) = true; } }
-      int const tbb = (np + TB_CK_THREADS - 1) / TB_CK_THREADS;
-      if (ck8) {
-        cudaFuncSetAttribute(traceback_ckpt_pairs_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tb_ck_smem(8)));
-        traceback_ckpt_pairs_kernel<8><<<tbb, TB_CK_THREADS, tb_ck_smem(8), c->stream>>>(c->sp2, queries->d, targets->d, d_pairs, np,
-            static_cast<const uint2 *>(c->dir.p), static_cast<const uint2 *>(c->bnd.p), static_cast<char *>(c->cigar_scratch.p), d_stats);
-        count_launch();
-      }
-      if (ck16) {
-        cudaFuncSetAttribute(traceback_ckpt_pairs_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tb_ck_smem(16)));
-        traceback_ckpt_pairs_kernel<16><<<tbb, TB_CK_THREADS, tb_ck_smem(16), c->stream>>>(c->sp2, queries->d, targets->d, d_pairs, np,
-            static_cast<const uint2 *>(c->dir.p), static_cast<const uint2 *>(c->bnd.p), static_cast<char *>(c->cigar_scratch.p), d_stats);
-        count_launch();
-      }
-      VSG_CUDA_OK(cudaEventRecord(c->ev_pool[3 * ci + 2], c->stream));
-      cigar_len_kernel<<<(np + 255) / 256, 256, 0, c->stream>>>(d_pairs, d_stats, np, static_cast<int64_t *>(c->cigar_len.p));
-      count_launch();
-      size_t tmp_bytes = 0;
-      cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, static_cast<int64_t *>(c->cigar_len.p),
-                                    static_cast<int64_t *>(c->cigar_offs.p), np, c->stream);
-      if ((rc = c->cub_tmp.reserve(tmp_bytes + 16)) != VSG_OK) { return rc; }
-      cub::DeviceScan::ExclusiveSum(c->cub_tmp.p, tmp_bytes, static_cast<int64_t *>(c->cigar_len.p),
-                                    static_cast<int64_t *>(c->cigar_offs.p), np, c->stream);
-      count_launch();
-      cigar_gather_kernel<<<np, 64, 0, c->stream>>>(d_pairs, np, queries->d, targets->d, d_stats,
-                                                    static_cast<int64_t *>(c->cigar_offs.p),
-                                                    static_cast<char *>(c->cigar_scratch.p), static_cast<char *>(c->cigar_dense.p));
-      count_launch();
-      std::vector<int64_t> h_offs(static_cast<size_t>(np)), h_lens(static_cast<size_t>(np));
-      VSG_CUDA_OK(cudaMemcpyAsync(h_offs.data(), c->cigar_offs.p, sizeof(int64_t) * np, cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaMemcpyAsync(h_lens.data(), c->cigar_len.p, sizeof(int64_t) * np, cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
-      int64_t const total = np > 0 ? h_offs[static_cast<size_t>(np) - 1] + h_lens[static_cast<size_t>(np) - 1] : 0;
-      std::vector<char> dense(static_cast<size_t>(total) + 1);
-      if (total > 0) {
-        VSG_CUDA_OK(cudaMemcpyAsync(dense.data(), c->cigar_dense.p, static_cast<size_t>(total), cudaMemcpyDeviceToHost, c->stream));
-        VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
-      }
-      for (int p = 0; p < np; p++) { cigars[static_cast<size_t>(hpairs[p].out)] = std::string(dense.data() + h_offs[static_cast<size_t>(p)]); }
-    }
-  }
+  // ---- collect: statistics home, the host-resolved pairs merged in, the caller's arrays filled ---------------------
   int h_rerun = 0;
   if (d_rerun != nullptr) { VSG_CUDA_OK(cudaMemcpyAsync(&h_rerun, d_rerun, sizeof(int), cudaMemcpyDeviceToHost, c->stream)); }
-  if (!plans.empty()) {
-    VSG_CUDA_OK(cudaMemcpyAsync(hs, d_stats, sizeof(int32_t) * VSG_STAT_WORDS * static_cast<size_t>(npairs), cudaMemcpyDeviceToHost, c->stream));
+  if (!plan.chunks.empty()) {
+    VSG_CUDA_OK(cudaMemcpyAsync(hs, c->stats.p, sizeof(int32_t) * VSG_STAT_WORDS * static_cast<size_t>(npairs), cudaMemcpyDeviceToHost, c->stream));
   }
   VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
   VSG_CUDA_OK(cudaGetLastError());
-  for (size_t ci = 0; ci < plans.size(); ci++) {
+  for (size_t ci = 0; ci < plan.chunks.size(); ci++) {
+    Chunk const & ch = plan.chunks[ci];
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, c->ev_pool[3 * ci], c->ev_pool[3 * ci + 1]) == cudaSuccess) { c->prof_fwd_ms += ms; }
     if (cudaEventElapsedTime(&ms, c->ev_pool[3 * ci + 1], c->ev_pool[3 * ci + 2]) == cudaSuccess) { c->prof_tb_ms += ms; }
-    c->prof_cells += plans[ci].cells; c->prof_fast += plans[ci].nfast; c->prof_exact += plans[ci].nexact;
-    c->prof_fwd_launches += static_cast<int64_t>(plans[ci].runs.size()) + (plans[ci].exact_count > 0 ? 1 : 0);
+    c->prof_cells += ch.cells; c->prof_fast += ch.nfast; c->prof_exact += ch.exact_count;
+    c->prof_fwd_launches += static_cast<int64_t>(ch.runs.size()) + (ch.exact_count > 0 ? 1 : 0);
   }
-  for (auto const & hp : host_pairs) { std::memcpy(hs + static_cast<size_t>(hp.slot) * VSG_STAT_WORDS, hp.st, sizeof(int32_t) * VSG_STAT_WORDS); }
+  for (auto const & hp : plan.host_pairs) { std::memcpy(hs + static_cast<size_t>(hp.slot) * VSG_STAT_WORDS, hp.st, sizeof(int32_t) * VSG_STAT_WORDS); }
 
   int64_t cpos = 0;
   for (int64_t k = 0; k < npairs; k++) {
     int32_t const * s = hs + static_cast<size_t>(k) * VSG_STAT_WORDS;
-    if (gated && leader_of[k] >= 0 && s[VSG_STAT_ALIGNED] == -1 && s[VSG_STAT_MATCHES] == -1) { c->prof_tb_skipped++; }
+    if (plan.gated && leader_of[k] >= 0 && s[VSG_STAT_ALIGNED] == -1 && s[VSG_STAT_MATCHES] == -1) { c->prof_tb_skipped++; }
     score[k] = static_cast<int16_t>(s[VSG_STAT_SCORE]);
     if (aligned != nullptr) { aligned[k] = static_cast<uint16_t>(s[VSG_STAT_ALIGNED]); }
     if (matches != nullptr) { matches[k] = static_cast<uint16_t>(s[VSG_STAT_MATCHES]); }
@@ -1087,7 +1076,7 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
       trims[4 * k + 3] = tr < 0 ? -tr : 0;
     }
     if (want_cigar) {
-      std::string const & cg = cigars[static_cast<size_t>(k)];
+      std::string const & cg = plan.cigars[static_cast<size_t>(k)];
       if (cpos + static_cast<int64_t>(cg.size()) + 1 > cigar_cap) { Error::set("vsg_align_pairs: cigar buffer too small"); return VSG_ECAP; }
       cigar_off[k] = cpos;
       std::memcpy(cigar_buf + cpos, cg.c_str(), cg.size() + 1);
@@ -1095,16 +1084,16 @@ int vsg::align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_se
     }
   }
   if (want_cigar) { cigar_off[npairs] = cpos; }
-  if (ck_counts != nullptr) { ck_counts[0] = n_stored; ck_counts[1] = n_scoreonly; ck_counts[2] = h_rerun; }
+  if (ck_counts != nullptr) { ck_counts[0] = plan.n_stored; ck_counts[1] = plan.n_scoreonly; ck_counts[2] = h_rerun; }
   if (trace) {
     auto const t_end = std::chrono::steady_clock::now();
     std::fprintf(stderr, "[vsg trace] align_pairs %lld pairs, %zu chunk(s): plan %.1f ms, total %.1f ms\n",
-                 static_cast<long long>(npairs), plans.size(),
+                 static_cast<long long>(npairs), plan.chunks.size(),
                  std::chrono::duration<double, std::milli>(t_planned - t_begin).count(),
                  std::chrono::duration<double, std::milli>(t_end - t_begin).count());
-    if (n_stored + n_scoreonly > 0) {
+    if (plan.n_stored + plan.n_scoreonly > 0) {
       std::fprintf(stderr, "[vsg trace] align_pairs checkpoint tasks: %lld stored, %lld score-only, %d of them re-run with stores\n",
-                   static_cast<long long>(n_stored), static_cast<long long>(n_scoreonly), h_rerun);
+                   static_cast<long long>(plan.n_stored), static_cast<long long>(plan.n_scoreonly), h_rerun);
     }
   }
   return VSG_OK;

@@ -58,11 +58,14 @@ struct ExactTask {
   uint64_t he_off;   // 2*qlen int16
 };
 
+// PairDesc::kind: where the pair's forward pass left what its traceback reads
+enum { PD_FAST = 0, PD_EXACT = 1, PD_CKPT = 2 };
+
 // What the traceback kernel needs to find a pair's direction bits.
 struct PairDesc {
   uint32_t q, t;
   uint64_t dir_off;
-  int32_t kind;   // 0 = fast layout, 1 = exact layout, 2 = checkpoints (align_ckpt.cuh): dir_off / aux_off are uint2 element offsets
+  int32_t kind;   // PD_FAST = fast layout, PD_EXACT = exact layout, PD_CKPT = checkpoints (align_ckpt.cuh): dir_off / aux_off are uint2 element offsets
   int32_t out;    // pair slot in the stats array
   int32_t R;      // fast: rows per lane
   int32_t half;   // fast: 0 = low nibble, 1 = high nibble; checkpoints: bit 0 = half, bit 1 = general alphabet
@@ -109,6 +112,15 @@ int align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_seqset 
                       uint16_t * mismatches, uint16_t * gaps, int32_t * trims,
                       char * cigar_buf, int64_t cigar_cap, int64_t * cigar_off,
                       const int32_t * leader_of, double gate_threshold, int gate_iddef, int64_t * ck_counts = nullptr);
+
+// owning handle of a sequence set
+struct SeqsetDeleter { void operator()(vsg_seqset * s) const { vsg_seqset_destroy(s); } };
+using SeqsetPtr = std::unique_ptr<vsg_seqset, SeqsetDeleter>;
+
+// the reverse complements of src's sequences [q0, q0 + n), as a compact set
+int seqset_revcomp(vsg_ctx * c, const vsg_seqset * src, int64_t q0, int64_t n, SeqsetPtr & out);
+// both strands of every sequence of src, sequence s at 2s and its reverse complement at 2s+1
+int seqset_both_strands(vsg_ctx * c, const vsg_seqset * src, SeqsetPtr & out);
 
 }  // namespace vsg
 
