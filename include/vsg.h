@@ -183,7 +183,8 @@ void vsg_index_destroy(vsg_index * ix);
  *      of `queries` in [q0, q0+nq).  For query q the best-first list (count desc, target length
  *      asc, target number asc) of at most tophits targets with count >= min(minwordmatches,
  *      number of distinct query k-mers) is written to cand_seqno/cand_count[(q-q0)*tophits ...],
- *      its length to ncand[q-q0].  Host pointers. ---- */
+ *      its length to ncand[q-q0].  Host pointers.  Any tophits >= 1: up to 1024 the lists are kept in shared
+ *      memory; above, every target at the threshold is counted, written out and sorted in device memory. ---- */
 int vsg_rank(vsg_ctx * ctx, const vsg_index * ix, const vsg_seqset * queries, int64_t q0,
              int64_t nq, int minwordmatches, int tophits, int mask_lower,
              uint32_t * cand_seqno, uint32_t * cand_count, int32_t * ncand);
@@ -271,6 +272,14 @@ int vsg_search_batch(vsg_ctx * ctx, const vsg_index * ix, const vsg_seqset * db,
                      const vsg_seqset * queries, int64_t q0, int64_t nq,
                      const vsg_search_opts * opts, vsg_search_result * results, int max_results,
                      int32_t * counts, int64_t * work);
+/* The same search with variable-length hit lists, for limits that leave a query thousands of hits (--maxaccepts 0
+ * --maxrejects 0: every target, usearch_global.cpp:598-614).  The rows of query q0+i are hits[first[i] .. first[i+1])
+ * (first: nq + 1 offsets), at most maxhits of them (0: all), in search_joinhits order: the rows vsg_search_batch gives
+ * with a large enough max_results.  *nhits receives the number of rows produced; if it exceeds cap the call returns
+ * VSG_ECAP with first filled and hits untouched.  work as for vsg_search_batch. */
+int vsg_search_hits(vsg_ctx * ctx, const vsg_index * ix, const vsg_seqset * db, const vsg_seqset * queries, int64_t q0,
+                    int64_t nq, const vsg_search_opts * opts, int64_t maxhits, vsg_search_result * hits, int64_t cap,
+                    int64_t * first, int64_t * nhits, int64_t * work);
 
 /* ---- all-against-all: replaces the per-query body of allpairs_thread_run
  *      (commands/allpairs_global.cpp:340-549) for query rows [row0, row0+nrows) of `set`: every
@@ -372,6 +381,10 @@ int vsg_group_set_fallback(vsg_group * g, vsg_fallback_fn fn, void * user);
 int vsg_group_search(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,
                      int dust_queries, const vsg_search_opts * opts, vsg_search_result * results, int max_results,
                      int32_t * counts, int64_t * work);
+/* vsg_group_search with the hit lists of vsg_search_hits: query i's rows are hits[first[i] .. first[i+1]) */
+int vsg_group_search_hits(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,
+                          int dust_queries, const vsg_search_opts * opts, int64_t maxhits, vsg_search_result * hits,
+                          int64_t cap, int64_t * first, int64_t * nhits, int64_t * work);
 int vsg_group_allpairs(vsg_group * g, const vsg_search_opts * opts, vsg_pair_hit * hits, int64_t cap,
                        int64_t * nhits, int64_t * work);
 

@@ -164,14 +164,13 @@ int slice_fallback(void * u, int64_t query, int32_t strand, int64_t target, int6
   SliceFallback const * w = static_cast<SliceFallback *>(u);
   return w->fn(w->user, query + w->base, strand, target, out);
 }
-}  // namespace
 
-extern "C" int vsg_group_search(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,
-                                int dust_queries, const vsg_search_opts * opts, vsg_search_result * results, int max_results,
-                                int32_t * counts, int64_t * work)
+// The queries of a group call sharded over the devices: fn(d, ctx, slice, b0, b1, opts, work4) searches queries
+// [b0, b1) of the call, uploaded (and DUST-masked) on device d as `slice`, with opts rebased to the slice.
+template <class Fn>
+int group_run(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq, int dust_queries,
+              const vsg_search_opts * opts, int64_t * work, Fn && fn)
 {
-  if (g == nullptr || opts == nullptr || results == nullptr || counts == nullptr || nq < 0 ||
-      (nq > 0 && (qcat == nullptr || qoff == nullptr || qlen == nullptr))) { Error::set("vsg_group_search: bad argument"); return VSG_EINVAL; }
   int const nd = static_cast<int>(g->ctx.size());
   if (work != nullptr) { work[0] = work[1] = work[2] = work[3] = 0; }
   if (nq == 0) { return VSG_OK; }
@@ -205,10 +204,7 @@ extern "C" int vsg_group_search(vsg_group * g, const char * qcat, const int64_t 
     vsg_search_opts o = *opts;
     if (o.query_sizes != nullptr) { o.query_sizes += b0; }
     if (o.query_labels != nullptr) { o.query_labels += b0; }
-    if (rc == VSG_OK) {
-      rc = vsg_search_batch(c, g->index[static_cast<size_t>(d)], g->db[static_cast<size_t>(d)], q, 0, b1 - b0, &o,
-                            results + static_cast<size_t>(b0) * max_results, max_results, counts + b0, w.data() + 4 * d);
-    }
+    if (rc == VSG_OK) { rc = fn(d, c, q, b0, b1, o, w.data() + 4 * d); }
     if (g->fallback != nullptr) { vsg_ctx_set_fallback(c, g->fallback, g->fallback_user); }
     if (q != nullptr) { vsg_seqset_destroy(q); }
     return rc;
@@ -218,6 +214,68 @@ extern "C" int vsg_group_search(vsg_group * g, const char * qcat, const int64_t 
     for (int z = 0; z < 4; z++) { work[z] += w[static_cast<size_t>(4 * d + z)]; }
   }
   return VSG_OK;
+}
+
+}  // namespace
+
+extern "C" int vsg_group_search(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,
+                                int dust_queries, const vsg_search_opts * opts, vsg_search_result * results, int max_results,
+                                int32_t * counts, int64_t * work)
+{
+  if (g == nullptr || opts == nullptr || results == nullptr || counts == nullptr || nq < 0 ||
+      (nq > 0 && (qcat == nullptr || qoff == nullptr || qlen == nullptr))) { Error::set("vsg_group_search: bad argument"); return VSG_EINVAL; }
+  return group_run(g, qcat, qoff, qlen, nq, dust_queries, opts, work,
+                   [&](int d, vsg_ctx * c, const vsg_seqset * q, int64_t b0, int64_t b1, const vsg_search_opts & o, int64_t * w) {
+    return vsg_search_batch(c, g->index[static_cast<size_t>(d)], g->db[static_cast<size_t>(d)], q, 0, b1 - b0, &o,
+                            results + static_cast<size_t>(b0) * max_results, max_results, counts + b0, w);
+  });
+}
+
+namespace vsg {
+
+int group_search_rows(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq, int dust_queries,
+                      const vsg_search_opts * opts, int64_t maxhits, std::vector<vsg_search_result> & rows,
+                      std::vector<int64_t> & first, int64_t * work)
+{
+  if (g == nullptr || opts == nullptr || nq < 0 || maxhits < 0 || (nq > 0 && (qcat == nullptr || qoff == nullptr || qlen == nullptr))) {
+    Error::set("vsg_group_search_hits: bad argument");
+    return VSG_EINVAL;
+  }
+  int const nd = static_cast<int>(g->ctx.size());
+  std::vector<std::vector<vsg_search_result>> drows(static_cast<size_t>(nd));
+  std::vector<std::vector<int64_t>> dfirst(static_cast<size_t>(nd));
+  int const rc = group_run(g, qcat, qoff, qlen, nq, dust_queries, opts, work,
+                           [&](int d, vsg_ctx * c, const vsg_seqset * q, int64_t b0, int64_t b1, const vsg_search_opts & o, int64_t * w) {
+    return search_hits_host(c, g->index[static_cast<size_t>(d)], g->db[static_cast<size_t>(d)], q, 0, b1 - b0, &o, maxhits,
+                            drows[static_cast<size_t>(d)], dfirst[static_cast<size_t>(d)], w);
+  });
+  if (rc != VSG_OK) { return rc; }
+  // the devices' slices are consecutive query ranges: concatenate them in device order
+  rows.clear();
+  first.assign(1, 0);
+  for (int d = 0; d < nd; d++) {
+    auto const & fd = dfirst[static_cast<size_t>(d)];
+    for (size_t i = 1; i < fd.size(); i++) { first.push_back(static_cast<int64_t>(rows.size()) + fd[i]); }
+    rows.insert(rows.end(), drows[static_cast<size_t>(d)].begin(), drows[static_cast<size_t>(d)].end());
+    std::vector<vsg_search_result>().swap(drows[static_cast<size_t>(d)]);
+  }
+  first.resize(static_cast<size_t>(nq) + 1, static_cast<int64_t>(rows.size()));
+  return VSG_OK;
+}
+
+}  // namespace vsg
+
+extern "C" int vsg_group_search_hits(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,
+                                     int dust_queries, const vsg_search_opts * opts, int64_t maxhits, vsg_search_result * hits,
+                                     int64_t cap, int64_t * first, int64_t * nhits, int64_t * work)
+{
+  if (first == nullptr || nhits == nullptr || cap < 0 || (cap > 0 && hits == nullptr)) { Error::set("vsg_group_search_hits: bad argument"); return VSG_EINVAL; }
+  *nhits = 0;
+  std::vector<vsg_search_result> rows;
+  std::vector<int64_t> f;
+  int const rc = group_search_rows(g, qcat, qoff, qlen, nq, dust_queries, opts, maxhits, rows, f, work);
+  if (rc != VSG_OK) { return rc; }
+  return hits_out(rows, f, "vsg_group_search_hits", hits, cap, first, nhits);
 }
 
 extern "C" int vsg_group_allpairs(vsg_group * g, const vsg_search_opts * opts, vsg_pair_hit * hits, int64_t cap,

@@ -18,7 +18,8 @@
 // of 16-byte vectors that the 16 warps split evenly (every lane busy every round) —, scans the counters against a
 // running threshold and appends the survivors as 64-bit sort keys to a candidate list that is sorted and cut to
 // `tophits` at the end (and whenever a crowd of ties fills it up).  HBM traffic per query is the postings themselves
-// (2 B each) — the counters never leave the SM.
+// (2 B each) — the counters never leave the SM.  Above TOPHITS_MAX candidates per query (rank_lists) the keys of every
+// target at the threshold go to HBM instead and are sorted there per query.
 #include "vsg_internal.h"
 
 #include <cub/cub.cuh>
@@ -35,7 +36,7 @@ constexpr int SHARD = 1 << SHARD_BITS;  // targets per shard
 constexpr int RANK_THREADS = 512;
 constexpr int KMER_CAP = 2048;          // distinct-k-mer capacity per query (query length <= 2047 + k)
 constexpr int CAND_CAP = 2048;          // candidate keys held in shared memory
-constexpr int TOPHITS_MAX = 1024;
+constexpr int TOPHITS_MAX = RANK_TOPHITS_MAX;
 constexpr int SCAN_SEG_WORDS = 512;     // counters are scanned 1024 at a time (<= 1024 new candidates)
 constexpr int COUNTER_WORDS = SHARD / 2 + 1;
 // Static index: a shard holds 32766 targets and its postings are stored as the BYTE OFFSET of the target's counter
@@ -267,12 +268,18 @@ __device__ __forceinline__ uint64_t make_key(uint32_t count, uint32_t len, uint3
          static_cast<uint64_t>(0xffffffu - seqno);
 }
 
-template <bool INCR>
+// RANK_TOP: the best `tophits` of every query in shared memory (tophits <= TOPHITS_MAX).  The unbounded path
+// (rank_lists) runs the same k-mer extraction and posting stream twice: RANK_COUNT writes to out_n how many targets of
+// each query reach the reference's threshold, RANK_EMIT writes their keys to keys[key_off[qi] ...] in no order.
+enum { RANK_TOP = 0, RANK_COUNT = 1, RANK_EMIT = 2 };
+
+template <bool INCR, int MODE = RANK_TOP>
 __global__ void __launch_bounds__(RANK_THREADS, 2)
 rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restrict__ shards, int nshards,
             int k, int mask_lower, int minwordmatches, int tophits,
             uint32_t * __restrict__ out_seqno, uint32_t * __restrict__ out_count, int32_t * __restrict__ out_n,
-            int32_t * __restrict__ status, uint32_t * __restrict__ scratch, size_t scratch_stride, int bitmap_words)
+            int32_t * __restrict__ status, uint32_t * __restrict__ scratch, size_t scratch_stride, int bitmap_words,
+            const int64_t * __restrict__ key_off, uint64_t * __restrict__ keys)
 {
   extern __shared__ __align__(16) unsigned char smem[];
   uint64_t * const cand = reinterpret_cast<uint64_t *>(smem);                     // CAND_CAP
@@ -373,7 +380,7 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
     // least `tophits` targets at or above it.  A target below T can never reach the final list, so
     // only counts >= T are turned into candidate keys: a few dozen per shard instead of the ~3 % of
     // all targets that pass the reference's fixed threshold (searchcore.cpp:320), no overflow sorts.
-    bool const running = !longq && (np2 + nk + 1 <= KMER_CAP);
+    bool const running = MODE == RANK_TOP && !longq && (np2 + nk + 1 <= KMER_CAP);
     uint32_t * const hist = kmers + np2;  // nk + 1 bins in the unused tail of the k-mer array
     if (running) {
       for (int i = threadIdx.x; i <= nk; i += blockDim.x) { hist[i] = 0; }
@@ -560,6 +567,19 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
       }  // chunk
       int const nwords = (S.nt + 1) >> 1;
       uint32_t thr = minmatches;
+      if constexpr (MODE != RANK_TOP) {
+        // 4u. every target at or above the threshold; the counters are cleared behind the scan
+        scan_counters(S.nt, minmatches, 1, [&](uint32_t c, int lt) {
+          int const pos = atomicAdd(&s_ncand, 1);
+          if (MODE == RANK_EMIT) {
+            int const t = S.t0 + lt;
+            keys[key_off[qi] + pos] = make_key(c, static_cast<uint32_t>(db.len[t]), static_cast<uint32_t>(t));
+          }
+        });
+        clean = true;
+        __syncthreads();
+        continue;  // next shard
+      }
       if (running) {
         // 4r. histogram of this shard's counts >= T, new T, then keys for counts >= new T only
         uint32_t const T0 = static_cast<uint32_t>(s_T);
@@ -673,6 +693,11 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
     }
     // 5. final order.  Usually far more targets pass the k-mer threshold than are wanted: find the
     //    count T of the tophits-th best with a histogram, keep count >= T, sort only those.
+    if constexpr (MODE != RANK_TOP) {
+      if (threadIdx.x == 0) { out_n[qi] = s_ncand; }
+      __syncthreads();
+      continue;  // next query
+    }
     int m = s_ncand;
     __syncthreads();
     if (running) {
@@ -1005,6 +1030,12 @@ namespace vsg {
 const vsg_seqset * index_db(const vsg_index * ix) { return ix->db; }
 int index_wordlength(const vsg_index * ix) { return ix->k; }
 
+template <int MODE>
+static int rank_launch(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
+                       int minwordmatches, int tophits, int mask_lower, uint32_t * d_seqno, uint32_t * d_count,
+                       int32_t * d_n, int32_t * d_status, const int64_t * d_key_off, uint64_t * d_keys);
+void rank_collect_time(vsg_ctx * c);
+
 // device-side results left in ctx->rank_tmp: [seqno nq*tophits][count nq*tophits][n nq][status 1]
 int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
                  int minwordmatches, int tophits, int mask_lower, uint32_t ** d_seqno, uint32_t ** d_count,
@@ -1023,8 +1054,19 @@ int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, 
   *d_status = *d_n + nq;
   VSG_CUDA_OK(cudaMemsetAsync(*d_status, 0, sizeof(int32_t), c->stream));
   if (nq == 0) { return VSG_OK; }
+  return rank_launch<RANK_TOP>(c, ix, queries, q0, nq, minwordmatches, tophits, mask_lower, *d_seqno, *d_count, *d_n,
+                               *d_status, nullptr, nullptr);
+}
+
+// the static-index ranker over queries [q0, q0 + nq) on c's stream, timed by ev[4..5]
+template <int MODE>
+static int rank_launch(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
+                       int minwordmatches, int tophits, int mask_lower, uint32_t * d_seqno, uint32_t * d_count,
+                       int32_t * d_n, int32_t * d_status, const int64_t * d_key_off, uint64_t * d_keys)
+{
+  int rc;
   cudaStream_t const rs = c->stream;
-  VSG_CUDA_OK(cudaFuncSetAttribute(rank_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(RANK_SMEM)));
+  VSG_CUDA_OK(cudaFuncSetAttribute(rank_kernel<false, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(RANK_SMEM)));
   int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
   int const grid = static_cast<int>(std::min<int64_t>(nq, static_cast<int64_t>(sms) * 2));
@@ -1041,13 +1083,127 @@ int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, 
     d_scratch = static_cast<uint32_t *>(c->rank_scratch.p);
   }
   VSG_CUDA_OK(cudaEventRecord(c->ev[4], rs));
-  rank_kernel<false><<<grid, RANK_THREADS, RANK_SMEM, rs>>>(
+  rank_kernel<false, MODE><<<grid, RANK_THREADS, RANK_SMEM, rs>>>(
       queries->d, q0, static_cast<int>(nq), ix->db->d, static_cast<const ShardDev *>(ix->b_shards.p),
-      static_cast<int>(ix->h_shards.size()), ix->k, mask_lower, minwordmatches, tophits, *d_seqno, *d_count, *d_n,
-      *d_status, d_scratch, stride, bitmap_words);
+      static_cast<int>(ix->h_shards.size()), ix->k, mask_lower, minwordmatches, tophits, d_seqno, d_count, d_n,
+      d_status, d_scratch, stride, bitmap_words, d_key_off, d_keys);
   count_launch();
   VSG_CUDA_OK(cudaEventRecord(c->ev[5], rs));
   c->rank_pending = true;
+  return VSG_OK;
+}
+
+// the first min(n, tophits) sorted keys of every query of a chunk as (target, count): one block per query
+__global__ void cut_lists_kernel(const uint64_t * __restrict__ keys, const int64_t * __restrict__ key_off,
+                                 const int64_t * __restrict__ out_off, uint32_t * __restrict__ seqno, uint32_t * __restrict__ count)
+{
+  int const q = blockIdx.x;
+  int64_t const a = key_off[q], n = out_off[q + 1] - out_off[q], o = out_off[q];
+  for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
+    uint64_t const key = keys[a + i];
+    seqno[o + i] = 0xffffffu - static_cast<uint32_t>(key & 0xffffffu);
+    count[o + i] = static_cast<uint32_t>(key >> 49);
+  }
+}
+
+// The count pass of the unbounded ranker: n[i] = the number of targets query q0 + i has at or above the reference's
+// threshold, min(minwordmatches, distinct k-mers) (its whole candidate list before any cut)
+int rank_counts(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                int mask_lower, std::vector<int32_t> & n)
+{
+  if (q0 < 0 || nq < 0 || q0 + nq > queries->d.n) { Error::set("vsg_rank: query range out of bounds"); return VSG_EINVAL; }
+  if (queries->device != c->device || ix->device != c->device) { Error::set("vsg_rank: sequence set / index lives on another device than the context"); return VSG_EINVAL; }
+  if (nq > (1 << 30)) { Error::set("vsg_rank: batch too large"); return VSG_EINVAL; }
+  n.assign(static_cast<size_t>(nq), 0);
+  if (nq == 0) { return VSG_OK; }
+  int rc;
+  if ((rc = c->rank_tmp.reserve(sizeof(int32_t) * (static_cast<size_t>(nq) + 4))) != VSG_OK) { return rc; }
+  int32_t * const d_n = static_cast<int32_t *>(c->rank_tmp.p);
+  int32_t * const d_status = d_n + nq;
+  VSG_CUDA_OK(cudaMemsetAsync(d_status, 0, sizeof(int32_t), c->stream));
+  if ((rc = rank_launch<RANK_COUNT>(c, ix, queries, q0, nq, minwordmatches, 1, mask_lower, nullptr, nullptr, d_n, d_status,
+                                    nullptr, nullptr)) != VSG_OK) { return rc; }
+  int32_t status = 0;
+  VSG_CUDA_OK(cudaMemcpyAsync(n.data(), d_n, sizeof(int32_t) * static_cast<size_t>(nq), cudaMemcpyDeviceToHost, c->stream));
+  VSG_CUDA_OK(cudaMemcpyAsync(&status, d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
+  rank_collect_time(c);
+  if (status != 0) {
+    Error::set("vsg_rank: a query is longer than the device ranker supports (65 534 + wordlength nt)");
+    return VSG_EINVAL;
+  }
+  return VSG_OK;
+}
+
+// The unbounded ranker (any tophits): query i's list is seqno / count[first[i] .. first[i + 1]), best first, the
+// targets with count >= min(minwordmatches, distinct k-mers) cut to tophits.  A count pass sizes every list; then, for
+// as many queries as the key budget holds at a time, an emit pass writes the keys, a segmented sort orders each
+// query's keys and cut_lists_kernel keeps the first tophits.  Keys, sort buffers and lists take 24 bytes per candidate
+// from a quarter of the context's direction-bit budget (a share of the device's free memory, vsg_ctx_create).  The
+// context's ranker time (vsg_profile.rank_ms) covers the count pass and, per chunk, the emit pass, sort and cut.
+int rank_lists(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+               int64_t tophits, int mask_lower, std::vector<int64_t> & first, std::vector<uint32_t> & seqno,
+               std::vector<uint32_t> & count)
+{
+  if (tophits < 1) { Error::set("vsg_rank: tophits must be at least 1"); return VSG_EINVAL; }
+  std::vector<int32_t> n;
+  int rc = rank_counts(c, ix, queries, q0, nq, minwordmatches, mask_lower, n);
+  if (rc != VSG_OK) { return rc; }
+  first.assign(static_cast<size_t>(nq) + 1, 0);
+  seqno.clear(); count.clear();
+  if (nq == 0) { return VSG_OK; }
+  int const th = static_cast<int>(std::min<int64_t>(tophits, INT32_MAX));
+  for (int64_t i = 0; i < nq; i++) { first[static_cast<size_t>(i) + 1] = first[static_cast<size_t>(i)] + std::min<int64_t>(n[static_cast<size_t>(i)], tophits); }
+  seqno.resize(static_cast<size_t>(first[static_cast<size_t>(nq)]));
+  count.resize(seqno.size());
+  // 2. chunks of consecutive queries whose keys fit the budget (one query at least)
+  int64_t const budget = std::min<int64_t>(static_cast<int64_t>(c->dir_budget / 4 / 24), INT32_MAX / 2);
+  std::vector<int64_t> koff, ooff;
+  for (int64_t a = 0; a < nq;) {
+    int64_t b = a, keys = 0;
+    while (b < nq && (b == a || keys + n[static_cast<size_t>(b)] <= budget)) { keys += n[static_cast<size_t>(b)]; b++; }
+    int64_t const m = b - a;
+    koff.assign(static_cast<size_t>(m) + 1, 0); ooff.assign(static_cast<size_t>(m) + 1, 0);
+    for (int64_t i = 0; i < m; i++) {
+      koff[static_cast<size_t>(i) + 1] = koff[static_cast<size_t>(i)] + n[static_cast<size_t>(a + i)];
+      ooff[static_cast<size_t>(i) + 1] = first[static_cast<size_t>(a + i) + 1] - first[static_cast<size_t>(a)];
+    }
+    int64_t const nout = ooff[static_cast<size_t>(m)];
+    if (keys > 0) {
+      size_t const offs_b = sizeof(int64_t) * 2 * (static_cast<size_t>(m) + 1);
+      size_t const keys_b = sizeof(uint64_t) * static_cast<size_t>(keys);
+      if ((rc = c->rank_tmp.reserve(offs_b + 2 * keys_b + sizeof(uint32_t) * (2 * static_cast<size_t>(nout) + static_cast<size_t>(m) + 4) + 64)) != VSG_OK) { return rc; }
+      int64_t * const d_koff = static_cast<int64_t *>(c->rank_tmp.p);
+      int64_t * const d_ooff = d_koff + m + 1;
+      uint64_t * const d_k0 = reinterpret_cast<uint64_t *>(d_ooff + m + 1);
+      uint64_t * const d_k1 = d_k0 + keys;
+      uint32_t * const d_seq = reinterpret_cast<uint32_t *>(d_k1 + keys);
+      uint32_t * const d_cnt = d_seq + nout;
+      int32_t * const d_n2 = reinterpret_cast<int32_t *>(d_cnt + nout);   // the emit pass's counts (not read back)
+      VSG_CUDA_OK(cudaMemcpyAsync(d_koff, koff.data(), sizeof(int64_t) * (static_cast<size_t>(m) + 1), cudaMemcpyHostToDevice, c->stream));
+      VSG_CUDA_OK(cudaMemcpyAsync(d_ooff, ooff.data(), sizeof(int64_t) * (static_cast<size_t>(m) + 1), cudaMemcpyHostToDevice, c->stream));
+      if ((rc = rank_launch<RANK_EMIT>(c, ix, queries, q0 + a, m, minwordmatches, th, mask_lower, nullptr, nullptr, d_n2, d_n2 + m,
+                                       d_koff, d_k0)) != VSG_OK) { return rc; }
+      cub::DoubleBuffer<uint64_t> db(d_k0, d_k1);
+      size_t tb = 0;
+      cub::DeviceSegmentedSort::SortKeysDescending(nullptr, tb, db, static_cast<int>(keys), static_cast<int>(m), d_koff, d_koff + 1, c->stream);
+      if ((rc = c->cub_tmp.reserve(tb + 64)) != VSG_OK) { return rc; }
+      cub::DeviceSegmentedSort::SortKeysDescending(c->cub_tmp.p, tb, db, static_cast<int>(keys), static_cast<int>(m), d_koff, d_koff + 1, c->stream);
+      count_launch();
+      if (nout > 0) {
+        cut_lists_kernel<<<static_cast<unsigned>(m), 256, 0, c->stream>>>(db.Current(), d_koff, d_ooff, d_seq, d_cnt);
+        count_launch();
+        VSG_CUDA_OK(cudaEventRecord(c->ev[5], c->stream));   // the chunk's ranker time runs from its emit pass to here
+        size_t const o = static_cast<size_t>(first[static_cast<size_t>(a)]);
+        VSG_CUDA_OK(cudaMemcpyAsync(seqno.data() + o, d_seq, sizeof(uint32_t) * static_cast<size_t>(nout), cudaMemcpyDeviceToHost, c->stream));
+        VSG_CUDA_OK(cudaMemcpyAsync(count.data() + o, d_cnt, sizeof(uint32_t) * static_cast<size_t>(nout), cudaMemcpyDeviceToHost, c->stream));
+      }
+      VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
+      VSG_CUDA_OK(cudaGetLastError());
+      rank_collect_time(c);
+    }
+    a = b;
+  }
   return VSG_OK;
 }
 
@@ -1071,6 +1227,19 @@ extern "C" int vsg_rank(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * qu
     return VSG_EINVAL;
   }
   VSG_CUDA_OK(cudaSetDevice(c->device));
+  if (tophits > TOPHITS_MAX) {
+    std::vector<int64_t> first;
+    std::vector<uint32_t> seqno, count;
+    int const rc = rank_lists(c, ix, queries, q0, nq, minwordmatches, tophits, mask_lower, first, seqno, count);
+    if (rc != VSG_OK) { return rc; }
+    for (int64_t i = 0; i < nq; i++) {
+      size_t const a = static_cast<size_t>(first[static_cast<size_t>(i)]), n = static_cast<size_t>(first[static_cast<size_t>(i) + 1]) - a;
+      std::memcpy(cand_seqno + static_cast<size_t>(i) * tophits, seqno.data() + a, sizeof(uint32_t) * n);
+      std::memcpy(cand_count + static_cast<size_t>(i) * tophits, count.data() + a, sizeof(uint32_t) * n);
+      ncand[i] = static_cast<int32_t>(n);
+    }
+    return VSG_OK;
+  }
   uint32_t *d_seqno, *d_count; int32_t *d_n, *d_status;
   int rc = rank_enqueue(c, ix, queries, q0, nq, minwordmatches, tophits, mask_lower, &d_seqno, &d_count, &d_n, &d_status);
   if (rc != VSG_OK) { return rc; }
@@ -1284,7 +1453,7 @@ int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, in
   }
   rank_kernel<true><<<grid, RANK_THREADS, RANK_SMEM, c->stream>>>(
       queries->d, q0, static_cast<int>(nq), lens, static_cast<const ShardDev *>(ix->b_shards.p), nshards, ix->k, ix->mask_lower,
-      minwordmatches, tophits, *d_seqno, *d_count, *d_n, *d_status, d_scratch, stride, bitmap_words);
+      minwordmatches, tophits, *d_seqno, *d_count, *d_n, *d_status, d_scratch, stride, bitmap_words, nullptr, nullptr);
   count_launch();
   return VSG_OK;
 }

@@ -23,12 +23,18 @@
 #include <cstring>
 #include <chrono>
 #include <cstdio>
+#include <functional>
 
 namespace vsg {
 int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
                  int minwordmatches, int tophits, int mask_lower, uint32_t ** d_seqno, uint32_t ** d_count,
                  int32_t ** d_n, int32_t ** d_status);
 void rank_collect_time(vsg_ctx * c);
+int rank_lists(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+               int64_t tophits, int mask_lower, std::vector<int64_t> & first, std::vector<uint32_t> & seqno,
+               std::vector<uint32_t> & count);
+int rank_counts(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                int mask_lower, std::vector<int32_t> & n);
 const vsg_seqset * index_db(const vsg_index * ix);
 int index_wordlength(const vsg_index * ix);
 }  // namespace vsg
@@ -44,7 +50,7 @@ struct QState {
   const uint32_t * cs = nullptr;
   const uint32_t * cc = nullptr;
   const uint8_t * cf = nullptr;  // per-candidate device verdicts of the sequence-content filters (0 = pass)
-  int hit_base = 0;  // index of this state's first Hit in the batch-wide hit array
+  int64_t hit_base = 0;  // index of this state's first Hit in the batch-wide hit array (room for ncand)
   int hit_count = 0, accepts = 0, rejects = 0, finalized = 0, delayed = 0;
   int gpos = -1;  // lazy mode: next hit of the open group to examine (-1: no group open)
   int gend = 0, greq = 0;  // lazy mode: end of the requested hit range, number of pairs requested
@@ -56,6 +62,9 @@ struct SearchScratch {  // per host thread, see vsg_ctx::search_scratch
   std::vector<uint32_t> h_seqno, h_count;
   std::vector<uint8_t> h_flags;
   std::vector<int32_t> h_n;
+  std::vector<int64_t> cfirst;   // state i's candidates are h_seqno / h_count / h_flags[cfirst[i] ...], h_n[i] of them
+  std::vector<int64_t> lfirst;   // unbounded ranker: one strand's lists (rank_lists)
+  std::vector<uint32_t> lseq, lcnt;
   std::vector<QState> st;
   Hit * hits = nullptr;
   size_t hits_cap = 0;
@@ -74,15 +83,25 @@ struct SearchScratch {  // per host thread, see vsg_ctx::search_scratch
 // idprefix / idsuffix / selfid of search_acceptable_unaligned (searchcore.cpp:588-607) for every candidate
 // of every query of a ranked batch: one warp per (query, candidate) compares 4-bit codes as seqcmp does
 // (utils/seqcmp.cpp:72-92).  flags: 1 = idprefix fails, 2 = idsuffix fails, 4 = selfid fails.
+// Candidate lists at a stride of tophits (ncand[qi] of them valid), or, with first != nullptr, back to back: query qi's
+// are cand[first[qi] .. first[qi + 1]).
 __global__ void prefilter_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const uint32_t * __restrict__ cand,
-                                 const int32_t * __restrict__ ncand, int tophits, int idprefix, int idsuffix, int selfid,
-                                 uint8_t * __restrict__ flags)
+                                 const int32_t * __restrict__ ncand, int tophits, const int64_t * __restrict__ first,
+                                 int idprefix, int idsuffix, int selfid, uint8_t * __restrict__ flags)
 {
   int64_t const w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   int const lane = threadIdx.x & 31;
-  if (w >= static_cast<int64_t>(nq) * tophits) { return; }
-  int const qi = static_cast<int>(w / tophits), j = static_cast<int>(w % tophits);
-  if (j >= ncand[qi]) { return; }
+  int qi;
+  if (first == nullptr) {
+    if (w >= static_cast<int64_t>(nq) * tophits) { return; }
+    qi = static_cast<int>(w / tophits);
+    if (static_cast<int>(w % tophits) >= ncand[qi]) { return; }
+  } else {
+    if (w >= first[nq]) { return; }
+    int lo = 0, hi = nq - 1;   // the last query whose list starts at or before w
+    while (lo < hi) { int const mid = (lo + hi + 1) >> 1; if (first[mid] <= w) { lo = mid; } else { hi = mid - 1; } }
+    qi = lo;
+  }
   uint32_t const t = cand[w];
   const uint8_t * __restrict__ q = qs.sym + qs.off[q0 + qi];
   const uint8_t * __restrict__ d = db.sym + db.off[t];
@@ -115,16 +134,28 @@ extern "C" void vsg_search_opts_default(vsg_search_opts * o)
   o->query_sizes = nullptr; o->target_sizes = nullptr; o->query_labels = nullptr; o->target_labels = nullptr;
 }
 
-extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * db,
-                                const vsg_seqset * queries, int64_t q0, int64_t nq,
-                                const vsg_search_opts * opts, vsg_search_result * results, int max_results,
-                                int32_t * counts, int64_t * work)
+namespace {
+
+// a joined hit list (search_joinhits order) of query q, the index within the call; called once per query, from the
+// driver's worker threads
+using RowSink = std::function<void(int64_t q, const std::vector<Hit> & joined)>;
+
+// the result record of a hit (search.cpp:466-488)
+vsg_search_result result_of(Hit const & h, int qlen, int tlen)
 {
-  if (c == nullptr || ix == nullptr || db == nullptr || queries == nullptr || opts == nullptr ||
-      results == nullptr || counts == nullptr || max_results < 1) {
-    Error::set("vsg_search_batch: bad argument");
-    return VSG_EINVAL;
-  }
+  vsg_search_result r;
+  r.target = h.target; r.matches = h.matches; r.mismatches = h.mismatches; r.gaps = h.nwgaps;
+  r.alignment_length = h.nwalignmentlength;
+  r.query_length = qlen;
+  r.target_length = tlen;
+  r.accepted = h.accepted ? 1 : 0; r.strand = h.strand; r.nwscore = h.nwscore; r.id = h.id;
+  r.internal_alignment_length = h.internal_alignmentlength; r.internal_gaps = h.internal_gaps;
+  return r;
+}
+
+int search_core(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * db, const vsg_seqset * queries, int64_t q0,
+                int64_t nq, const vsg_search_opts * opts, RowSink const & sink, int64_t * work)
+{
   if (index_db(ix) != db) { Error::set("vsg_search_batch: index was built for another sequence set"); return VSG_EINVAL; }
   if (q0 < 0 || nq < 0 || q0 + nq > queries->d.n) { Error::set("vsg_search_batch: query range out of bounds"); return VSG_EINVAL; }
   if (opts->wordlength != index_wordlength(ix)) { Error::set("vsg_search_batch: wordlength differs from the index"); return VSG_EINVAL; }
@@ -156,10 +187,10 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
               opts->maxid == d.maxid && opts->mid == d.mid && opts->iddef >= 0 && opts->iddef <= 4 && opt_weak_id <= opt_id &&
               opts->unoise == 0;
   }
-  for (int64_t q = 0; q < nq; q++) { counts[q] = 0; }
   if (seqcount == 0 || nq == 0) { if (work) { work[0] = work[1] = work[2] = work[3] = 0; } return VSG_OK; }
-  if (lim.tophits > 1024) { Error::set("vsg_search_batch: maxaccepts+maxrejects+8 > 1024 is not supported on the device ranker"); return VSG_EINVAL; }
-  int const tophits = static_cast<int>(lim.tophits);
+  // tophits beyond what the ranker keeps in shared memory: the unbounded ranker's lists
+  bool const unbounded = lim.tophits > RANK_TOPHITS_MAX;
+  int const tophits = static_cast<int>(std::min<int64_t>(lim.tophits, RANK_TOPHITS_MAX));
   int const nstrands = opts->strand_both ? 2 : 1;
   if (opts->self != 0 && (opts->query_labels == nullptr || opts->target_labels == nullptr)) {
     Error::set("vsg_search_batch: --self needs query_labels and target_labels"); return VSG_EINVAL;
@@ -172,7 +203,34 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
   // others keep the GPU busy.  Results land in disjoint slots, so no ordering is needed.
   int64_t BATCH = 4096;
   if (const char * e = std::getenv("VSG_SUBBATCH")) { BATCH = std::max<int64_t>(256, std::atoll(e)); }
-  int64_t const nbatches = (nq + BATCH - 1) / BATCH;
+  // With the unbounded lists the host holds every candidate of a sub-batch at once: its list entry, its hit slot and, in
+  // the round that aligns it, its pair (about 200 bytes each).  Such sub-batches are therefore cut from the ranker's
+  // count pass by candidate volume, both strands counted: at most SUBBATCH_CANDIDATES (about 0.8 GB of host memory each,
+  // a few GB for the sub-batches of all host threads in flight) and at most BATCH queries; a query with more candidates
+  // than that is a sub-batch of its own.
+  constexpr int64_t SUBBATCH_CANDIDATES = int64_t(1) << 22;
+  std::vector<int64_t> pieces;   // unbounded: sub-batch i is queries [pieces[i], pieces[i + 1])
+  if (unbounded) {
+    std::vector<int32_t> n, nrc;
+    if (int const r = rank_counts(c, ix, queries, q0, nq, lim.minwordmatches, opts->mask_lower, n); r != VSG_OK) { return r; }
+    if (nstrands == 2) {
+      SeqsetPtr rc_all;
+      int r = seqset_revcomp(c, queries, q0, nq, rc_all);
+      if (r == VSG_OK && opts->qmask_dust != 0) { r = vsg_seqset_dust(c, rc_all.get()); }
+      if (r == VSG_OK) { r = rank_counts(c, ix, rc_all.get(), 0, nq, lim.minwordmatches, opts->mask_lower, nrc); }
+      if (r != VSG_OK) { return r; }
+    }
+    pieces.push_back(0);
+    int64_t vol = 0;
+    for (int64_t q = 0; q < nq; q++) {
+      int64_t v = std::min<int64_t>(n[static_cast<size_t>(q)], lim.tophits);
+      if (nstrands == 2) { v += std::min<int64_t>(nrc[static_cast<size_t>(q)], lim.tophits); }
+      if (q > pieces.back() && (vol + v > SUBBATCH_CANDIDATES || q - pieces.back() >= BATCH)) { pieces.push_back(q); vol = 0; }
+      vol += v;
+    }
+    pieces.push_back(nq);
+  }
+  int64_t const nbatches = unbounded ? static_cast<int64_t>(pieces.size()) - 1 : (nq + BATCH - 1) / BATCH;
   int nthreads = 8;
   if (const char * e = std::getenv("VSG_HOST_THREADS")) { nthreads = std::max(1, std::atoi(e)); }
   nthreads = static_cast<int>(std::min<int64_t>(nthreads, nbatches));
@@ -188,7 +246,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
   if (!c->search_scratch) { c->search_scratch = std::make_shared<SearchScratch>(); }
   SearchScratch & sc = *static_cast<SearchScratch *>(c->search_scratch.get());
   auto & st = sc.st;
-  Hit *& hits = sc.hits;  // bn*nstrands*tophits slots, deliberately uninitialised (each is zeroed when popped)
+  Hit *& hits = sc.hits;  // one slot per candidate of the sub-batch, deliberately uninitialised (each is zeroed when popped)
   auto & pq = sc.pq; auto & pt = sc.pt;
   auto & pstate = sc.pstate;  // which state each pair belongs to
   auto & px = sc.px;          // which of the state's hits
@@ -214,43 +272,85 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
       // reverse complement inherited from the masked plus strand does not matter
       if (opts->qmask_dust != 0 && (r = vsg_seqset_dust(c, rc_set.get())) != VSG_OK) { return r; }
     }
-    size_t const cells = static_cast<size_t>(bn) * tophits;
-    sc.h_seqno.resize(cells * nstrands); sc.h_count.resize(cells * nstrands); sc.h_n.resize(static_cast<size_t>(bn) * nstrands);
-    if (content_filters) { sc.h_flags.resize(cells * nstrands); }
-    for (int s = 0; s < nstrands; s++) {
-      uint32_t *d_seqno, *d_count; int32_t *d_n, *d_status;
-      const vsg_seqset * qset = (s == 0) ? queries : rc_set.get();
-      int64_t const qq0 = (s == 0) ? q0 + b0 : 0;
-      int r = rank_enqueue(c, ix, qset, qq0, bn, lim.minwordmatches, tophits, opts->mask_lower, &d_seqno, &d_count, &d_n, &d_status);
-      if (r != VSG_OK) { return r; }
-      int32_t status = 0;
-      VSG_CUDA_OK(cudaMemcpyAsync(sc.h_seqno.data() + cells * s, d_seqno, sizeof(uint32_t) * cells, cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaMemcpyAsync(sc.h_count.data() + cells * s, d_count, sizeof(uint32_t) * cells, cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaMemcpyAsync(sc.h_n.data() + bn * s, d_n, sizeof(int32_t) * bn, cudaMemcpyDeviceToHost, c->stream));
-      if (content_filters) {
-        if ((r = c->pre_flags.reserve(cells + 16)) != VSG_OK) { return r; }
-        VSG_CUDA_OK(cudaMemsetAsync(c->pre_flags.p, 0, cells, c->stream));
-        int64_t const nwarps = bn * tophits;
-        prefilter_kernel<<<static_cast<unsigned>((nwarps * 32 + 255) / 256), 256, 0, c->stream>>>(
-            qset->d, qq0, static_cast<int>(bn), db->d, d_seqno, d_n, tophits, opts->idprefix, opts->idsuffix, opts->selfid,
-            static_cast<uint8_t *>(c->pre_flags.p));
-        count_launch();
-        VSG_CUDA_OK(cudaMemcpyAsync(sc.h_flags.data() + cells * s, c->pre_flags.p, cells, cudaMemcpyDeviceToHost, c->stream));
+    size_t const nst = static_cast<size_t>(bn) * nstrands;
+    auto & cfirst = sc.cfirst;
+    cfirst.assign(nst + 1, 0);
+    sc.h_n.resize(nst);
+    if (unbounded) {
+      // lists back to back, each as long as the query's candidates (up to tophits)
+      sc.h_seqno.clear(); sc.h_count.clear(); sc.h_flags.clear();
+      for (int s = 0; s < nstrands; s++) {
+        const vsg_seqset * qset = (s == 0) ? queries : rc_set.get();
+        int64_t const qq0 = (s == 0) ? q0 + b0 : 0;
+        int r = rank_lists(c, ix, qset, qq0, bn, lim.minwordmatches, lim.tophits, opts->mask_lower, sc.lfirst, sc.lseq, sc.lcnt);
+        if (r != VSG_OK) { return r; }
+        int64_t const base = static_cast<int64_t>(sc.h_seqno.size());
+        for (int64_t q = 0; q < bn; q++) {
+          size_t const i = static_cast<size_t>(s) * bn + q;
+          cfirst[i] = base + sc.lfirst[static_cast<size_t>(q)];
+          sc.h_n[i] = static_cast<int32_t>(sc.lfirst[static_cast<size_t>(q) + 1] - sc.lfirst[static_cast<size_t>(q)]);
+        }
+        sc.h_seqno.insert(sc.h_seqno.end(), sc.lseq.begin(), sc.lseq.end());
+        sc.h_count.insert(sc.h_count.end(), sc.lcnt.begin(), sc.lcnt.end());
+        if (content_filters) {
+          size_t const n = sc.lseq.size();
+          sc.h_flags.resize(sc.h_seqno.size(), 0);
+          if (n == 0) { continue; }
+          size_t const fb = sizeof(int64_t) * (static_cast<size_t>(bn) + 1);
+          if ((r = c->rank_tmp.reserve(fb + sizeof(uint32_t) * n + 16)) != VSG_OK || (r = c->pre_flags.reserve(n + 16)) != VSG_OK) { return r; }
+          int64_t * const d_first = static_cast<int64_t *>(c->rank_tmp.p);
+          uint32_t * const d_cand = reinterpret_cast<uint32_t *>(d_first + bn + 1);
+          VSG_CUDA_OK(cudaMemcpyAsync(d_first, sc.lfirst.data(), fb, cudaMemcpyHostToDevice, c->stream));
+          VSG_CUDA_OK(cudaMemcpyAsync(d_cand, sc.lseq.data(), sizeof(uint32_t) * n, cudaMemcpyHostToDevice, c->stream));
+          prefilter_kernel<<<static_cast<unsigned>((static_cast<int64_t>(n) * 32 + 255) / 256), 256, 0, c->stream>>>(
+              qset->d, qq0, static_cast<int>(bn), db->d, d_cand, nullptr, 0, d_first, opts->idprefix, opts->idsuffix, opts->selfid,
+              static_cast<uint8_t *>(c->pre_flags.p));
+          count_launch();
+          VSG_CUDA_OK(cudaMemcpyAsync(sc.h_flags.data() + base, c->pre_flags.p, n, cudaMemcpyDeviceToHost, c->stream));
+          VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
+        }
       }
-      VSG_CUDA_OK(cudaMemcpyAsync(&status, d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
-      rank_collect_time(c);
-      if (status != 0) {
-        Error::set("vsg_search_batch: a query is longer than the device ranker supports (65 534 + wordlength nt)");
-        return VSG_EINVAL;
+    } else {
+      size_t const cells = static_cast<size_t>(bn) * tophits;
+      for (size_t i = 0; i < nst; i++) { cfirst[i] = static_cast<int64_t>(i) * tophits; }
+      sc.h_seqno.resize(cells * nstrands); sc.h_count.resize(cells * nstrands);
+      if (content_filters) { sc.h_flags.resize(cells * nstrands); }
+      for (int s = 0; s < nstrands; s++) {
+        uint32_t *d_seqno, *d_count; int32_t *d_n, *d_status;
+        const vsg_seqset * qset = (s == 0) ? queries : rc_set.get();
+        int64_t const qq0 = (s == 0) ? q0 + b0 : 0;
+        int r = rank_enqueue(c, ix, qset, qq0, bn, lim.minwordmatches, tophits, opts->mask_lower, &d_seqno, &d_count, &d_n, &d_status);
+        if (r != VSG_OK) { return r; }
+        int32_t status = 0;
+        VSG_CUDA_OK(cudaMemcpyAsync(sc.h_seqno.data() + cells * s, d_seqno, sizeof(uint32_t) * cells, cudaMemcpyDeviceToHost, c->stream));
+        VSG_CUDA_OK(cudaMemcpyAsync(sc.h_count.data() + cells * s, d_count, sizeof(uint32_t) * cells, cudaMemcpyDeviceToHost, c->stream));
+        VSG_CUDA_OK(cudaMemcpyAsync(sc.h_n.data() + bn * s, d_n, sizeof(int32_t) * bn, cudaMemcpyDeviceToHost, c->stream));
+        if (content_filters) {
+          if ((r = c->pre_flags.reserve(cells + 16)) != VSG_OK) { return r; }
+          VSG_CUDA_OK(cudaMemsetAsync(c->pre_flags.p, 0, cells, c->stream));
+          int64_t const nwarps = bn * tophits;
+          prefilter_kernel<<<static_cast<unsigned>((nwarps * 32 + 255) / 256), 256, 0, c->stream>>>(
+              qset->d, qq0, static_cast<int>(bn), db->d, d_seqno, d_n, tophits, nullptr, opts->idprefix, opts->idsuffix, opts->selfid,
+              static_cast<uint8_t *>(c->pre_flags.p));
+          count_launch();
+          VSG_CUDA_OK(cudaMemcpyAsync(sc.h_flags.data() + cells * s, c->pre_flags.p, cells, cudaMemcpyDeviceToHost, c->stream));
+        }
+        VSG_CUDA_OK(cudaMemcpyAsync(&status, d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+        VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
+        rank_collect_time(c);
+        if (status != 0) {
+          Error::set("vsg_search_batch: a query is longer than the device ranker supports (65 534 + wordlength nt)");
+          return VSG_EINVAL;
+        }
       }
     }
 
     t_rank += ms(tp0, now()); tp0 = now();
-    // one state per (query, strand); hits preallocated at tophits per state
-    st.assign(static_cast<size_t>(bn) * nstrands, QState());
+    // one state per (query, strand); a hit slot per candidate
+    st.assign(nst, QState());
     {
-      size_t const need = static_cast<size_t>(bn) * nstrands * tophits;
+      size_t need = 0;
+      for (size_t i = 0; i < nst; i++) { st[i].hit_base = static_cast<int64_t>(need); need += static_cast<size_t>(sc.h_n[i]); }
       if (need > sc.hits_cap) {
         std::free(hits);
         hits = static_cast<Hit *>(std::malloc(sizeof(Hit) * need));
@@ -263,16 +363,27 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
         QState & S = st[static_cast<size_t>(s) * bn + q];
         S.strand = s; S.ql = q;
         S.qlen = s == 0 ? queries->h_len[static_cast<size_t>(q0 + b0 + q)] : rc_set->h_len[static_cast<size_t>(q)];
-        S.ncand = sc.h_n[static_cast<size_t>(s) * bn + q];
-        S.cs = sc.h_seqno.data() + cells * s + static_cast<size_t>(q) * tophits;
-        S.cc = sc.h_count.data() + cells * s + static_cast<size_t>(q) * tophits;
-        S.cf = content_filters ? sc.h_flags.data() + cells * s + static_cast<size_t>(q) * tophits : nullptr;
-        S.hit_base = static_cast<int>((static_cast<size_t>(s) * bn + q) * tophits);
+        size_t const i = static_cast<size_t>(s) * bn + q;
+        S.ncand = sc.h_n[i];
+        S.cs = sc.h_seqno.data() + cfirst[i];
+        S.cc = sc.h_count.data() + cfirst[i];
+        S.cf = content_filters ? sc.h_flags.data() + cfirst[i] : nullptr;
       }
     }
+    // True when every candidate the state has left will be examined: neither limit nor the guard of the candidate loop
+    // can be reached before its list ends, because each hit examined adds one accept or one reject.  Then none of that
+    // work is speculative, and the state's whole remaining list is one group, aligned in one device call instead of
+    // eight candidates per round; the pairs aligned and the decisions are those of the groups of eight.  (Applied with
+    // the unbounded ranker's lists, where a query can have thousands of candidates.)
+    auto exhaustible = [&](QState const & S) -> bool {
+      int64_t const left = S.ncand - S.finalized;
+      return unbounded && left > MAXDELAYED && S.accepts + left <= maxaccepts && S.rejects + left <= maxrejects &&
+             S.ncand <= maxaccepts + maxrejects - 1;
+    };
     // search_onequery's candidate loop (searchcore.cpp:915-954) up to its next align_delayed; false when the
     // query's search has ended.  search_acceptable_unaligned (searchcore.cpp:541-609) pre-rejects candidates.
     auto next_group = [&](QState & S) -> bool {
+      bool const whole = exhaustible(S);
       while ((S.finalized + S.delayed < maxaccepts + maxrejects - 1) && (S.rejects < maxrejects) &&
              (S.accepts < maxaccepts) && (S.next < S.ncand)) {
         Hit & h = hits[static_cast<size_t>(S.hit_base) + S.hit_count];
@@ -289,7 +400,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
           h.rejected = true;
         }
         S.hit_count++;
-        if (S.delayed == MAXDELAYED) { return true; }
+        if (S.delayed == MAXDELAYED && !whole) { return true; }
       }
       if (S.delayed == 0) { S.done = true; return false; }
       return true;
@@ -520,18 +631,7 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
         }
       }
       std::stable_sort(joined.begin(), joined.end(), hit_less);
-      int const n = static_cast<int>(std::min<size_t>(joined.size(), static_cast<size_t>(max_results)));
-      for (int j = 0; j < n; j++) {
-        Hit const & h = joined[static_cast<size_t>(j)];
-        vsg_search_result & r = results[static_cast<size_t>(b0 + q) * max_results + j];
-        r.target = h.target; r.matches = h.matches; r.mismatches = h.mismatches; r.gaps = h.nwgaps;
-        r.alignment_length = h.nwalignmentlength;
-        r.query_length = queries->h_len[static_cast<size_t>(q0 + b0 + q)];
-        r.target_length = db->h_len[static_cast<size_t>(h.target)];
-        r.accepted = h.accepted ? 1 : 0; r.strand = h.strand; r.nwscore = h.nwscore; r.id = h.id;
-        r.internal_alignment_length = h.internal_alignmentlength; r.internal_gaps = h.internal_gaps;
-      }
-      counts[b0 + q] = n;
+      sink(b0 + q, joined);
     }
     t_join += ms(tp0, now());
   }
@@ -547,6 +647,15 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
   std::vector<int64_t> tp(static_cast<size_t>(nthreads), 0), tc(static_cast<size_t>(nthreads), 0), ap(static_cast<size_t>(nthreads), 0), ac(static_cast<size_t>(nthreads), 0);
   int const rc = run_parallel(nthreads, [&](int t) -> int {
     vsg_ctx * wc = c->children[static_cast<size_t>(t)];
+    if (unbounded) {   // the sub-batches cut above, in order
+      for (;;) {
+        int64_t const i = next.fetch_add(1);
+        if (i >= nbatches) { return VSG_OK; }
+        int64_t const b0 = pieces[static_cast<size_t>(i)], bn = pieces[static_cast<size_t>(i) + 1] - b0;
+        int const r = run_batch(wc, b0, bn, tp[static_cast<size_t>(t)], tc[static_cast<size_t>(t)], ap[static_cast<size_t>(t)], ac[static_cast<size_t>(t)]);
+        if (r != VSG_OK) { next.store(nbatches); return r; }
+      }
+    }
     // Sub-batches are cut from a shared cursor.  A thread's FIRST one is shortened to (t+1)/nthreads of
     // the regular size: identical sub-batches started together run in lockstep (all threads rank, then
     // all gather on the host, then all align ...) and the device idles through every host phase;
@@ -570,6 +679,82 @@ extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seq
   }
   if (work != nullptr) { work[0] = total_pairs; work[1] = total_cells; work[2] = aligned_pairs; work[3] = aligned_cells; }
   return VSG_OK;
+}
+
+}  // namespace
+
+extern "C" int vsg_search_batch(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * db,
+                                const vsg_seqset * queries, int64_t q0, int64_t nq,
+                                const vsg_search_opts * opts, vsg_search_result * results, int max_results,
+                                int32_t * counts, int64_t * work)
+{
+  if (c == nullptr || ix == nullptr || db == nullptr || queries == nullptr || opts == nullptr ||
+      results == nullptr || counts == nullptr || max_results < 1) {
+    Error::set("vsg_search_batch: bad argument");
+    return VSG_EINVAL;
+  }
+  for (int64_t q = 0; q < nq; q++) { counts[q] = 0; }
+  return search_core(c, ix, db, queries, q0, nq, opts, [&](int64_t q, const std::vector<Hit> & joined) {
+    int const n = static_cast<int>(std::min<size_t>(joined.size(), static_cast<size_t>(max_results)));
+    int const qlen = queries->h_len[static_cast<size_t>(q0 + q)];
+    for (int j = 0; j < n; j++) {
+      Hit const & h = joined[static_cast<size_t>(j)];
+      results[static_cast<size_t>(q) * max_results + j] = result_of(h, qlen, db->h_len[static_cast<size_t>(h.target)]);
+    }
+    counts[q] = n;
+  }, work);
+}
+
+namespace vsg {
+
+int search_hits_host(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * db, const vsg_seqset * queries, int64_t q0,
+                     int64_t nq, const vsg_search_opts * opts, int64_t maxhits, std::vector<vsg_search_result> & rows,
+                     std::vector<int64_t> & first, int64_t * work)
+{
+  if (c == nullptr || ix == nullptr || db == nullptr || queries == nullptr || opts == nullptr || nq < 0 || maxhits < 0) {
+    Error::set("vsg_search_hits: bad argument");
+    return VSG_EINVAL;
+  }
+  std::vector<std::vector<vsg_search_result>> perq(static_cast<size_t>(nq));
+  int const rc = search_core(c, ix, db, queries, q0, nq, opts, [&](int64_t q, const std::vector<Hit> & joined) {
+    size_t const n = maxhits > 0 ? std::min<size_t>(joined.size(), static_cast<size_t>(maxhits)) : joined.size();
+    int const qlen = queries->h_len[static_cast<size_t>(q0 + q)];
+    auto & out = perq[static_cast<size_t>(q)];
+    out.reserve(n);
+    for (size_t j = 0; j < n; j++) { out.push_back(result_of(joined[j], qlen, db->h_len[static_cast<size_t>(joined[j].target)])); }
+  }, work);
+  if (rc != VSG_OK) { return rc; }
+  first.assign(static_cast<size_t>(nq) + 1, 0);
+  for (int64_t q = 0; q < nq; q++) { first[static_cast<size_t>(q) + 1] = first[static_cast<size_t>(q)] + static_cast<int64_t>(perq[static_cast<size_t>(q)].size()); }
+  rows.clear();
+  rows.reserve(static_cast<size_t>(first[static_cast<size_t>(nq)]));
+  for (auto & v : perq) { rows.insert(rows.end(), v.begin(), v.end()); }
+  return VSG_OK;
+}
+
+int hits_out(const std::vector<vsg_search_result> & rows, const std::vector<int64_t> & first, const char * caller,
+             vsg_search_result * hits, int64_t cap, int64_t * first_out, int64_t * nhits)
+{
+  std::memcpy(first_out, first.data(), sizeof(int64_t) * first.size());
+  *nhits = static_cast<int64_t>(rows.size());
+  if (*nhits > cap) { Error::set(std::string(caller) + ": hit buffer too small"); return VSG_ECAP; }
+  if (!rows.empty()) { std::memcpy(hits, rows.data(), sizeof(vsg_search_result) * rows.size()); }
+  return VSG_OK;
+}
+
+}  // namespace vsg
+
+extern "C" int vsg_search_hits(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * db, const vsg_seqset * queries, int64_t q0,
+                               int64_t nq, const vsg_search_opts * opts, int64_t maxhits, vsg_search_result * hits, int64_t cap,
+                               int64_t * first, int64_t * nhits, int64_t * work)
+{
+  if (first == nullptr || nhits == nullptr || cap < 0 || (cap > 0 && hits == nullptr)) { Error::set("vsg_search_hits: bad argument"); return VSG_EINVAL; }
+  *nhits = 0;
+  std::vector<vsg_search_result> rows;
+  std::vector<int64_t> f;
+  int const rc = search_hits_host(c, ix, db, queries, q0, nq, opts, maxhits, rows, f, work);
+  if (rc != VSG_OK) { return rc; }
+  return hits_out(rows, f, "vsg_search_hits", hits, cap, first, nhits);
 }
 
 

@@ -103,6 +103,9 @@ struct PinBuf {
 
 void count_launch(int n = 1);
 
+// the most candidates per query the ranker keeps in shared memory (rank.cu); longer lists go through rank_lists
+constexpr int RANK_TOPHITS_MAX = 1024;
+
 // vsg_align_pairs with traceback on demand (align_ckpt.cuh, TbGate): leader_of[k] = index of pair k's group leader in
 // this call, or -1; threshold = 100 * --id (+ margin); skipped pairs return aligned = matches = mismatches = 0xffff.
 // ck_counts (optional, 3 entries): checkpoint tasks stored, score-only, re-run with stores
@@ -112,6 +115,19 @@ int align_pairs_gated(vsg_ctx * c, const vsg_seqset * queries, const vsg_seqset 
                       uint16_t * mismatches, uint16_t * gaps, int32_t * trims,
                       char * cigar_buf, int64_t cigar_cap, int64_t * cigar_off,
                       const int32_t * leader_of, double gate_threshold, int gate_iddef, int64_t * ck_counts = nullptr);
+
+// vsg_search_hits with the rows kept on the host: query i's are rows[first[i] .. first[i + 1]) (search.cu)
+int search_hits_host(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * db, const vsg_seqset * queries, int64_t q0,
+                     int64_t nq, const vsg_search_opts * opts, int64_t maxhits, std::vector<vsg_search_result> & rows,
+                     std::vector<int64_t> & first, int64_t * work);
+// vsg_group_search_hits with the rows kept on the host (group.cu)
+int group_search_rows(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq, int dust_queries,
+                      const vsg_search_opts * opts, int64_t maxhits, std::vector<vsg_search_result> & rows,
+                      std::vector<int64_t> & first, int64_t * work);
+// rows / first to the caller's buffers of vsg_search_hits / vsg_group_search_hits: *nhits = rows needed, VSG_ECAP
+// (first filled, hits untouched) when they exceed cap
+int hits_out(const std::vector<vsg_search_result> & rows, const std::vector<int64_t> & first, const char * caller,
+             vsg_search_result * hits, int64_t cap, int64_t * first_out, int64_t * nhits);
 
 // owning handle of a sequence set
 struct SeqsetDeleter { void operator()(vsg_seqset * s) const { vsg_seqset_destroy(s); } };

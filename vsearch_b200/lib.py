@@ -332,6 +332,33 @@ class Context:
                                        _ptr(work, C.c_int64)), "vsg_search_batch")
         return res, counts, work
 
+    def search_hits(self, ix: IndexHandle, db: SeqSetHandle, qs: SeqSetHandle, q0: int, nq: int,
+                    opts: SearchOpts, maxhits: int = 0, cap: Optional[int] = None):
+        """vsg_search_hits -> (rows, first[nq + 1], work[4]); query i's rows are rows[first[i]:first[i + 1]].
+        cap=None: the buffer is sized by a first call that reports the number of rows (VSG_ECAP) — that call runs the
+        whole search, so cap=None costs two searches; pass the row count when it is known (e.g. to time one search)."""
+        return _hits_call(lambda hits, c, first, n, work: load().vsg_search_hits(
+            self.h, ix.h, db.h, qs.h, C.c_int64(q0), C.c_int64(nq), C.byref(opts), C.c_int64(maxhits), hits, C.c_int64(c),
+            first, n, work), nq, cap, "vsg_search_hits")
+
+
+def _hits_call(call, nq: int, cap: Optional[int], what: str):
+    """a vsg_*search_hits call with a buffer of `cap` rows; cap=None: sized by a first call with cap 0 (VSG_ECAP), which
+    runs the whole search once more"""
+    first = np.zeros(nq + 1, dtype=np.int64)
+    work = np.zeros(4, dtype=np.int64)
+    n = C.c_int64()
+    if cap is None:
+        rc = call(None, 0, _ptr(first, C.c_int64), C.byref(n), _ptr(work, C.c_int64))
+        if rc == 0:
+            return (SearchResult * 0)(), first, work
+        if rc != -5:
+            _check(rc, what)
+        cap = int(n.value)
+    hits = (SearchResult * max(cap, 1))()
+    _check(call(hits, cap, _ptr(first, C.c_int64), C.byref(n), _ptr(work, C.c_int64)), what)
+    return hits, first, work
+
 
 def allpairs(ctx: "Context", ss: SeqSetHandle, row0: int, nrows: int, opts: SearchOpts, cap: int):
     """vsg_allpairs -> (numpy structured array of hits, work[2])"""
@@ -456,6 +483,16 @@ class Group:
                                        C.c_int64(nq), C.c_int(dust_queries), C.byref(opts), res, C.c_int(max_results),
                                        _ptr(counts, C.c_int32), _ptr(work, C.c_int64)), "vsg_group_search")
         return res, counts, work
+
+    def search_hits(self, qs, opts: SearchOpts, maxhits: int = 0, dust_queries: int = 0, cap: Optional[int] = None):
+        """vsg_group_search_hits -> (rows, first[nq + 1], work[4]), as Context.search_hits (cap=None: two searches)"""
+        nq = len(qs)
+        cat = np.ascontiguousarray(qs.cat, dtype=np.uint8)
+        offs = np.ascontiguousarray(qs.offs, dtype=np.int64)
+        lens = np.ascontiguousarray(qs.lens, dtype=np.int32)
+        return _hits_call(lambda hits, c, first, n, work: load().vsg_group_search_hits(
+            self.h, _ptr(cat, C.c_char), _ptr(offs, C.c_int64), _ptr(lens, C.c_int32), C.c_int64(nq), C.c_int(dust_queries),
+            C.byref(opts), C.c_int64(maxhits), hits, C.c_int64(c), first, n, work), nq, cap, "vsg_group_search_hits")
 
     def allpairs(self, opts: SearchOpts, cap: int):
         dt = np.dtype([("query", np.int32), ("target", np.int32), ("matches", np.int32), ("mismatches", np.int32),
