@@ -161,7 +161,10 @@ def test_multi_shard_database_vs_oracle(ctx):
 
 def test_ranker_ties_and_thresholds_vs_oracle(ctx):
     """the ranker's running threshold: thousands of targets tied on the k-mer count (more than its key
-    buffer holds), few candidates (< tophits), tophits from 1 to 1024, in one and in several shards"""
+    buffer holds), few candidates (< tophits), tophits from 1 to 1024, in one and in several shards.  The root
+    embedded in longer random queries takes the fixed-threshold scan instead: more survivors than the key buffer
+    holds (sort and cut per segment), the final histogram cut, and (2 600 nt) the same with the k-mers
+    de-duplicated in HBM"""
     rng = np.random.default_rng(53)
     root = synth.random_seqs(rng, 1, 150)[0]
     seqs = []
@@ -176,6 +179,11 @@ def test_ranker_ties_and_thresholds_vs_oracle(ctx):
     dbs = synth.SeqSet(seqs)
     queries = [root.tobytes(), synth.mutate(rng, root, 0.04).tobytes(), root[:60].tobytes(),
                other[5].tobytes(), synth.random_seqs(rng, 1, 120)[0].tobytes()]
+    for total in (1200, 2055, 2600):   # 2 055 nt: exactly the 2 048 windows the shared-memory k-mer path holds
+        left = (total - 150) // 2
+        flanks = synth.random_seqs(rng, 2, total - 150 - left)
+        queries.append(np.concatenate([flanks[0][:left], root, flanks[1]]).tobytes())
+    assert [len(q) for q in queries[-3:]] == [1200, 2055, 2600]
     qss = synth.SeqSet(queries)
     db = ctx.seqset(dbs); qs = ctx.seqset(qss)
     ix = ctx.index(db, 8, 0)

@@ -27,16 +27,6 @@
 #include <cstring>
 #include <string>
 
-namespace vsg {
-struct CIndex;
-int cindex_create(vsg_ctx * c, const vsg_seqset * set, int wordlength, int mask_lower, CIndex ** out);
-void cindex_destroy(CIndex * ix);
-int cindex_append(vsg_ctx * c, CIndex * ix, const uint32_t * seqnos, int n);
-int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
-                        int tophits, uint32_t ** d_seqno, uint32_t ** d_count, int32_t ** d_n, int32_t ** d_status);
-const std::vector<uint32_t> & cindex_seqnos(const CIndex * ix);
-}  // namespace vsg
-
 using namespace vsg;
 
 namespace {
@@ -195,15 +185,9 @@ int session_rounds(vsg_cluster_session & s, int64_t const start, int64_t const c
     size_t const cells = static_cast<size_t>(nst) * tophits;
     h_seqno.resize(cells); h_count.resize(cells); h_n.resize(static_cast<size_t>(nst));
     {
-      uint32_t *d_seqno, *d_count; int32_t *d_n, *d_status;
-      if ((rc = cindex_rank_enqueue(c, ix, qset, qi0, nst, minwordmatches, tophits, &d_seqno, &d_count, &d_n, &d_status)) != VSG_OK) { return rc; }
-      int32_t status = 0;
-      VSG_CUDA_OK(cudaMemcpyAsync(h_seqno.data(), d_seqno, sizeof(uint32_t) * cells, cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaMemcpyAsync(h_count.data(), d_count, sizeof(uint32_t) * cells, cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaMemcpyAsync(h_n.data(), d_n, sizeof(int32_t) * nst, cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaMemcpyAsync(&status, d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-      VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
-      if (status != 0) { Error::set("vsg_cluster_fast: a sequence is longer than the device ranker supports (65 534 + wordlength nt)"); return VSG_EINVAL; }
+      RankTop rt;
+      if ((rc = cindex_rank_enqueue(c, ix, qset, qi0, nst, minwordmatches, tophits, rt)) != VSG_OK ||
+          (rc = rank_download(c, rt, nst, tophits, h_seqno.data(), h_count.data(), h_n.data(), "vsg_cluster_fast")) != VSG_OK) { return rc; }
     }
     t_rank += ms_since(tp); tp = now();
     for (int u = 0; u < nst; u++) {

@@ -25,20 +25,6 @@
 #include <cstdio>
 #include <functional>
 
-namespace vsg {
-int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
-                 int minwordmatches, int tophits, int mask_lower, uint32_t ** d_seqno, uint32_t ** d_count,
-                 int32_t ** d_n, int32_t ** d_status);
-void rank_collect_time(vsg_ctx * c);
-int rank_lists(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
-               int64_t tophits, int mask_lower, std::vector<int64_t> & first, std::vector<uint32_t> & seqno,
-               std::vector<uint32_t> & count);
-int rank_counts(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
-                int mask_lower, std::vector<int32_t> & n);
-const vsg_seqset * index_db(const vsg_index * ix);
-int index_wordlength(const vsg_index * ix);
-}  // namespace vsg
-
 using namespace vsg;
 
 namespace {
@@ -316,32 +302,23 @@ int search_core(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * db, const 
       sc.h_seqno.resize(cells * nstrands); sc.h_count.resize(cells * nstrands);
       if (content_filters) { sc.h_flags.resize(cells * nstrands); }
       for (int s = 0; s < nstrands; s++) {
-        uint32_t *d_seqno, *d_count; int32_t *d_n, *d_status;
         const vsg_seqset * qset = (s == 0) ? queries : rc_set.get();
         int64_t const qq0 = (s == 0) ? q0 + b0 : 0;
-        int r = rank_enqueue(c, ix, qset, qq0, bn, lim.minwordmatches, tophits, opts->mask_lower, &d_seqno, &d_count, &d_n, &d_status);
+        RankTop rt;
+        int r = rank_enqueue(c, ix, qset, qq0, bn, lim.minwordmatches, tophits, opts->mask_lower, rt);
         if (r != VSG_OK) { return r; }
-        int32_t status = 0;
-        VSG_CUDA_OK(cudaMemcpyAsync(sc.h_seqno.data() + cells * s, d_seqno, sizeof(uint32_t) * cells, cudaMemcpyDeviceToHost, c->stream));
-        VSG_CUDA_OK(cudaMemcpyAsync(sc.h_count.data() + cells * s, d_count, sizeof(uint32_t) * cells, cudaMemcpyDeviceToHost, c->stream));
-        VSG_CUDA_OK(cudaMemcpyAsync(sc.h_n.data() + bn * s, d_n, sizeof(int32_t) * bn, cudaMemcpyDeviceToHost, c->stream));
         if (content_filters) {
           if ((r = c->pre_flags.reserve(cells + 16)) != VSG_OK) { return r; }
           VSG_CUDA_OK(cudaMemsetAsync(c->pre_flags.p, 0, cells, c->stream));
           int64_t const nwarps = bn * tophits;
           prefilter_kernel<<<static_cast<unsigned>((nwarps * 32 + 255) / 256), 256, 0, c->stream>>>(
-              qset->d, qq0, static_cast<int>(bn), db->d, d_seqno, d_n, tophits, nullptr, opts->idprefix, opts->idsuffix, opts->selfid,
+              qset->d, qq0, static_cast<int>(bn), db->d, rt.seqno, rt.n, tophits, nullptr, opts->idprefix, opts->idsuffix, opts->selfid,
               static_cast<uint8_t *>(c->pre_flags.p));
           count_launch();
           VSG_CUDA_OK(cudaMemcpyAsync(sc.h_flags.data() + cells * s, c->pre_flags.p, cells, cudaMemcpyDeviceToHost, c->stream));
         }
-        VSG_CUDA_OK(cudaMemcpyAsync(&status, d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
-        VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
-        rank_collect_time(c);
-        if (status != 0) {
-          Error::set("vsg_search_batch: a query is longer than the device ranker supports (65 534 + wordlength nt)");
-          return VSG_EINVAL;
-        }
+        if ((r = rank_download(c, rt, bn, tophits, sc.h_seqno.data() + cells * s, sc.h_count.data() + cells * s,
+                               sc.h_n.data() + bn * s, "vsg_search_batch")) != VSG_OK) { return r; }
       }
     }
 

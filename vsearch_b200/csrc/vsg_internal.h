@@ -103,8 +103,46 @@ struct PinBuf {
 
 void count_launch(int n = 1);
 
-// the most candidates per query the ranker keeps in shared memory (rank.cu); longer lists go through rank_lists
+// ---------------------------------------------------------------------------------------------
+// The k-mer ranker and its indexes (rank.cu)
+// ---------------------------------------------------------------------------------------------
+// the most candidates per query the ranker keeps in shared memory; longer lists go through rank_lists
 constexpr int RANK_TOPHITS_MAX = 1024;
+
+// The bounded ranker's results on the device, in ctx->rank_tmp: query i's candidates are seqno / count[i * tophits ...],
+// n[i] of them, best first; status != 0 when a query was too long to rank.
+struct RankTop {
+  uint32_t * seqno;
+  uint32_t * count;
+  int32_t * n;
+  int32_t * status;
+};
+
+const vsg_seqset * index_db(const vsg_index * ix);
+int index_wordlength(const vsg_index * ix);
+// enqueues the ranker over queries [q0, q0 + nq) on c's stream, timed into vsg_profile.rank_ms
+int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
+                 int minwordmatches, int tophits, int mask_lower, RankTop & out);
+// copies the results of rank_enqueue / cindex_rank_enqueue to the host, waits for them and checks their status
+int rank_download(vsg_ctx * c, const RankTop & r, int64_t nq, int tophits, uint32_t * h_seqno, uint32_t * h_count,
+                  int32_t * h_n, const char * caller);
+// unbounded ranker (any tophits): query i's list is seqno / count[first[i] .. first[i + 1])
+int rank_lists(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+               int64_t tophits, int mask_lower, std::vector<int64_t> & first, std::vector<uint32_t> & seqno,
+               std::vector<uint32_t> & count);
+// n[i] = how many targets query q0 + i has at or above the reference's threshold
+int rank_counts(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                int mask_lower, std::vector<int32_t> & n);
+
+// the cluster driver's incremental index of the centroids; candidates are DENSE target numbers (cindex_seqnos maps
+// them to sequence numbers)
+struct CIndex;
+int cindex_create(vsg_ctx * c, const vsg_seqset * set, int wordlength, int mask_lower, CIndex ** out);
+void cindex_destroy(CIndex * ix);
+int cindex_append(vsg_ctx * c, CIndex * ix, const uint32_t * seqnos, int n);
+int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                        int tophits, RankTop & out);
+const std::vector<uint32_t> & cindex_seqnos(const CIndex * ix);
 
 // vsg_align_pairs with traceback on demand (align_ckpt.cuh, TbGate): leader_of[k] = index of pair k's group leader in
 // this call, or -1; threshold = 100 * --id (+ margin); skipped pairs return aligned = matches = mismatches = 0xffff.
