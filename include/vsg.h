@@ -430,6 +430,43 @@ int vsg_udb_words(const vsg_udb * udb, const uint32_t ** kmercount, const uint32
 int vsg_udb_load(vsg_ctx * ctx, const vsg_udb * udb, vsg_seqset ** db, vsg_index ** index, int * mask_lower);
 int vsg_group_create_udb(const int * devices, int ndev, const vsg_scoring * scoring, const vsg_udb * udb, vsg_group ** out);
 
+/* ---- SINTAX taxonomy classification: replaces sintax_query / sintax_search_topscores / sintax_analyse
+ *      (commands/sintax.cpp:138-516) for --sintax with --randseed.  vsg_sintax runs the 100 bootstraps of every query
+ *      of `queries` in [q0, q0 + nq) and of its reverse complement (strand_both) against an index made by
+ *      vsg_index_create / vsg_udb_load: per strand, the distinct k-mers of the query in first-occurrence order (no
+ *      masking but non-ACGTU; unique_count, core/unique.cpp:155-353), 32 draws per bootstrap from one SplitMix64
+ *      generator per query seeded with random_substream_seed(seed, query number) (utils/random.cpp:70-91, plus strand
+ *      first, minus strand continuing its stream), and per bootstrap the target with the most sampled k-mers (ties:
+ *      shorter, then lower number), kept when its count is > 1.  out[i] belongs to query q0 + i.  A strand with fewer
+ *      than 32 distinct k-mers has no bootstraps.  The database must hold what db.read keeps for --sintax: sequences of
+ *      at least 32 nt (core/db.cpp minseqlength).  vsg_sintax_rows needs no device: the --tabbedout rows of nq results
+ *      (the vote over the winners' tax= fields, core/tax.cpp:70-186), written back to back into buf; *len receives
+ *      the bytes needed, VSG_ECAP (buf untouched) when they exceed cap.  target_headers are the full database headers
+ *      (--notrunclabels, as --sintax reads them).  vsg_sintax_stream is the --sintax command over a FASTA file: reader
+ *      thread, vsg_sintax on every device of the group, rows in input order from a writer thread; the input number of
+ *      the first record is 0.  random_ties (--sintax_random) is not offered: VSG_EINVAL, as is a cutoff outside 0..1.
+ *      ---- */
+#define VSG_SINTAX_BOOTSTRAPS 100
+typedef struct vsg_sintax_opts {
+  uint64_t seed;          /* --randseed; with --randseed 0 the caller draws a seed */
+  int64_t query_number0;  /* input number of queries[q0]: query q0 + i uses substream query_number0 + i (vsg_sintax) */
+  int32_t strand_both;    /* --strand both */
+  int32_t random_ties;    /* --sintax_random: not offered, VSG_EINVAL */
+  double cutoff;          /* --sintax_cutoff, 0..1 (rows only) */
+} vsg_sintax_opts;
+typedef struct vsg_sintax_result {
+  int32_t strand;                           /* chosen strand: 0 plus, 1 minus (sintax.cpp:480-507) */
+  int32_t nboot[2];                         /* successful bootstraps per strand */
+  int32_t best_count[2];                    /* largest winning k-mer count per strand */
+  int32_t seqno[2][VSG_SINTAX_BOOTSTRAPS];  /* winners per strand in bootstrap order, [0, nboot[s]); -1 beyond */
+} vsg_sintax_result;
+int vsg_sintax(vsg_ctx * ctx, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
+               const vsg_sintax_opts * opts, vsg_sintax_result * out);
+int vsg_sintax_rows(const vsg_sintax_result * results, int64_t nq, const char * const * query_headers,
+                    const char * const * target_headers, const vsg_sintax_opts * opts, char * buf, int64_t cap, int64_t * len);
+int vsg_sintax_stream(vsg_group * g, const char * const * target_headers, const char * query_fasta,
+                      const vsg_sintax_opts * opts, int batch_queries, const char * tabbedout_path, vsg_stream_stats * stats);
+
 #ifdef __cplusplus
 }
 #endif

@@ -263,6 +263,18 @@ int group_search_rows(vsg_group * g, const char * qcat, const int64_t * qoff, co
   return VSG_OK;
 }
 
+int group_sintax(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,
+                 const vsg_sintax_opts * opts, vsg_sintax_result * out)
+{
+  vsg_search_opts const none{};   // group_run's search options: no per-query arrays to rebase
+  return group_run(g, qcat, qoff, qlen, nq, 0, &none, nullptr,
+                   [&](int d, vsg_ctx * c, const vsg_seqset * q, int64_t b0, int64_t b1, const vsg_search_opts &, int64_t *) {
+    vsg_sintax_opts o = *opts;
+    o.query_number0 += b0;   // this device's first query keeps its input number
+    return vsg_sintax(c, g->index[static_cast<size_t>(d)], q, 0, b1 - b0, &o, out + b0);
+  });
+}
+
 }  // namespace vsg
 
 extern "C" int vsg_group_search_hits(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,

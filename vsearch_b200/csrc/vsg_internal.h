@@ -120,6 +120,9 @@ struct RankTop {
 
 const vsg_seqset * index_db(const vsg_index * ix);
 int index_wordlength(const vsg_index * ix);
+// the index's shards on its device (rank_steps.cuh)
+struct ShardDev;
+const ShardDev * index_shards(const vsg_index * ix, int & nshards);
 // enqueues the ranker over queries [q0, q0 + nq) on c's stream, timed into vsg_profile.rank_ms
 int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
                  int minwordmatches, int tophits, int mask_lower, RankTop & out);
@@ -162,6 +165,14 @@ int search_hits_host(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * db, c
 int group_search_rows(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq, int dust_queries,
                       const vsg_search_opts * opts, int64_t maxhits, std::vector<vsg_search_result> & rows,
                       std::vector<int64_t> & first, int64_t * work);
+// vsg_sintax of host queries sharded over the group's devices; query i gets input number opts->query_number0 + i
+int group_sintax(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,
+                 const vsg_sintax_opts * opts, vsg_sintax_result * out);
+// VSG_EINVAL (message prefixed with caller) for --sintax_random or a cutoff outside 0..1 (sintax.cu)
+int sintax_check_opts(const vsg_sintax_opts * o, const char * caller);
+// the --tabbedout rows of vsg_sintax_rows, appended to `out` (sintax.cu)
+int sintax_rows_string(const vsg_sintax_result * res, int64_t nq, const char * const * qheads, const char * const * theads,
+                       const vsg_sintax_opts * opts, std::string & out);
 // rows / first to the caller's buffers of vsg_search_hits / vsg_group_search_hits: *nhits = rows needed, VSG_ECAP
 // (first filled, hits untouched) when they exceed cap
 int hits_out(const std::vector<vsg_search_result> & rows, const std::vector<int64_t> & first, const char * caller,

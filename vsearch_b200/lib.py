@@ -322,6 +322,16 @@ class Context:
                                _ptr(count, C.c_uint32), _ptr(nc, C.c_int32)), "vsg_rank")
         return seqno, count, nc
 
+    def sintax(self, ix: IndexHandle, qs: SeqSetHandle, q0: int, nq: int, seed: int, strand_both: int = 0,
+               query_number0: Optional[int] = None, random_ties: int = 0):
+        """vsg_sintax -> dict of numpy arrays: strand[nq], nboot[nq, 2], best_count[nq, 2], seqno[nq, 2, 100] (-1 beyond
+        nboot); query q0 + i uses random substream query_number0 + i (default: q0 + i)"""
+        o = sintax_opts(seed, strand_both, query_number0=q0 if query_number0 is None else query_number0, random_ties=random_ties)
+        res = np.zeros(nq, dtype=SINTAX_DT)
+        _check(load().vsg_sintax(self.h, ix.h, qs.h, C.c_int64(q0), C.c_int64(nq), C.byref(o),
+                                 res.ctypes.data_as(C.c_void_p) if nq > 0 else None), "vsg_sintax")
+        return {k: res[k] for k in SINTAX_DT.names}
+
     def search(self, ix: IndexHandle, db: SeqSetHandle, qs: SeqSetHandle, q0: int, nq: int,
                opts: SearchOpts, max_results: int):
         res = (SearchResult * (nq * max_results))()
@@ -514,6 +524,52 @@ class Group:
                                          C.c_int(batch_queries), C.c_int64(maxhits), C.c_int(output_no_hits), blast6out.encode(),
                                          C.byref(st)), "vsg_usearch_stream")
         return {k: getattr(st, k) for k, _ in StreamStats._fields_}
+
+    def sintax_stream(self, target_headers, query_fasta: str, tabbedout: str, seed: int, strand_both: int = 0,
+                      cutoff: float = 0.0, batch_queries: int = 65536, random_ties: int = 0):
+        """vsg_sintax_stream: the --sintax command, FASTA file in, --tabbedout file out; returns the statistics as a dict"""
+        st = StreamStats()
+        o = sintax_opts(seed, strand_both, cutoff, random_ties=random_ties)
+        _check(load().vsg_sintax_stream(self.h, _strings(target_headers), query_fasta.encode(), C.byref(o), C.c_int(batch_queries),
+                                        tabbedout.encode(), C.byref(st)), "vsg_sintax_stream")
+        return {k: getattr(st, k) for k, _ in StreamStats._fields_}
+
+
+class SintaxOpts(C.Structure):
+    _fields_ = [("seed", C.c_uint64), ("query_number0", C.c_int64), ("strand_both", C.c_int32), ("random_ties", C.c_int32),
+                ("cutoff", C.c_double)]
+
+
+SINTAX_BOOTSTRAPS = 100
+SINTAX_DT = np.dtype([("strand", np.int32), ("nboot", np.int32, (2,)), ("best_count", np.int32, (2,)),
+                      ("seqno", np.int32, (2, SINTAX_BOOTSTRAPS))])
+
+
+def sintax_opts(seed: int, strand_both: int = 0, cutoff: float = 0.0, query_number0: int = 0, random_ties: int = 0) -> SintaxOpts:
+    return SintaxOpts(seed=seed, query_number0=query_number0, strand_both=strand_both, random_ties=random_ties, cutoff=cutoff)
+
+
+def _strings(xs):
+    return (C.c_char_p * len(xs))(*[x if isinstance(x, bytes) else x.encode() for x in xs])
+
+
+def sintax_rows(results: np.ndarray, query_headers, target_headers, cutoff: float = 0.0, strand_both: int = 0,
+                random_ties: int = 0) -> bytes:
+    """vsg_sintax_rows (host only, no device): the --tabbedout rows of a SINTAX_DT array of results"""
+    res = np.ascontiguousarray(results, dtype=SINTAX_DT)
+    o = sintax_opts(0, strand_both, cutoff, random_ties=random_ties)
+    qh, th = _strings(query_headers), _strings(target_headers)
+    n = C.c_int64()
+    rp = res.ctypes.data_as(C.c_void_p) if res.shape[0] > 0 else None
+    rc = load().vsg_sintax_rows(rp, C.c_int64(res.shape[0]), qh, th, C.byref(o), None, C.c_int64(0), C.byref(n))
+    if rc == 0:
+        return b""
+    if rc != -5:
+        _check(rc, "vsg_sintax_rows")
+    buf = C.create_string_buffer(int(n.value))
+    _check(load().vsg_sintax_rows(rp, C.c_int64(res.shape[0]), qh, th, C.byref(o), buf, C.c_int64(n.value), C.byref(n)),
+           "vsg_sintax_rows")
+    return buf.raw[: n.value]
 
 
 class UdbInfo(C.Structure):

@@ -160,3 +160,122 @@ def config2_query_batch(dbm: np.ndarray, n_q: int, q_len: int = 250, div: float 
     cols = start[:, None] + np.arange(q_len)[None, :]
     win = dbm[src[:, None], cols]
     return mutate_batch(rng, win, div), src
+
+
+# ---- SINTAX: a taxonomy database and amplicon-shaped queries ------------------------------------------------------------
+SINTAX_LEVELS = "dpcofgs"
+_RC = bytes.maketrans(b"ACGTacgtNn", b"TGCAtgcaNn")
+
+
+def revcomp(s: bytes) -> bytes:
+    return s.translate(_RC)[::-1]
+
+
+def sintax_data(seed: int = 77, length: int = 1450, fanout=(2, 2, 2, 2, 2, 2, 3), n_q: int = 300, q_len: int = 250):
+    """A reference tree of ranks d, p, c, o, f, g, s: every node is a mutation of its parent (rates falling from 10 % at
+    the domain to 2 % at the species), the species are ~`length`-nt leaves, and one species per genus is held out of
+    the database.  The database (headers ``r{i};tax=d:...,s:...;``) also holds the header variants of tax_parse /
+    tax_split (tax= not preceded by ';', no trailing ';', upper-case level letters, missing levels, a ',' after the tax
+    field), an exact duplicate with another taxonomy (ties broken by sequence number), a copy one base longer placed
+    first (ties broken by length), species with lower-case low-complexity stretches (so that --dbmask changes the
+    index) and one record under 32 nt (which --sintax drops).  Queries: mutated `q_len`-nt windows, 30 % of them
+    reverse-complemented, some from held-out species, some random, the low-complexity regions in upper case, a few with
+    fewer than 32 distinct k-mers (one of 10 nt), IUPAC and lower-case symbols, and two longer than 2 100 nt.
+    Returns dict(db_heads, db_seqs, q_heads, q_seqs, meta)."""
+    rng = np.random.default_rng(seed)
+    rates = (0.10, 0.08, 0.06, 0.05, 0.04, 0.03, 0.02)
+    leaves, held = [], []   # (names per level, sequence)
+
+    def grow(seq, names, level):
+        if level == len(SINTAX_LEVELS):
+            leaves.append((names, seq))
+            return
+        n = fanout[level] + (1 if level == len(SINTAX_LEVELS) - 1 else 0)
+        for j in range(n):
+            child = mutate(rng, seq, rates[level])
+            nm = names + [f"{SINTAX_LEVELS[level].upper()}{len(leaves) if level == 6 else ''}{'_'.join(names[-1:])}x{j}"]
+            if level == len(SINTAX_LEVELS) - 1 and j == n - 1:
+                held.append((nm, child))
+            else:
+                grow(child, nm, level + 1)
+
+    grow(random_seqs(rng, 1, length)[0], [], 0)
+    lc = set(range(3, len(leaves), 17))   # species with low-complexity stretches
+    db_heads, db_seqs = [], []
+    for i, (names, s) in enumerate(leaves):
+        seq = s.tobytes()
+        if i in lc:
+            unit = bytes(ACGT[rng.integers(0, 4, size=int(rng.integers(2, 4)))])
+            stretch = (unit * 200)[:180].lower()
+            p = int(rng.integers(100, len(seq) - 400))
+            seq = seq[:p] + stretch + seq[p + 180:]
+        db_seqs.append(seq)
+        tax = ",".join(f"{SINTAX_LEVELS[l]}:{names[l]}" for l in range(len(SINTAX_LEVELS)))
+        db_heads.append(f"r{i};tax={tax};")
+    # header variants
+    n = len(db_heads)
+    db_heads[1] = db_heads[1].replace(";tax=", ";size=3;tax=").rstrip(";")                       # no trailing ';'
+    db_heads[2] = "r2 xtax=d:Fake;" + db_heads[2][3:]                                            # tax= after 'x' skipped
+    db_heads[4] = db_heads[4].replace("d:", "D:").replace("g:", "G:")                          # upper-case levels
+    db_heads[5] = ",".join(p for p in db_heads[5].split(",") if not p.startswith(("c:", "o:")))  # missing levels
+    db_heads[6] = db_heads[6] + "note=a,b"                                                       # ',' after the field
+    # an exact duplicate with another species name (ties by number), and a copy one base longer placed before the
+    # original (ties by length): both of species 8 / 9, whose windows become queries below
+    dup_of, long_of = 8, 9
+    db_heads.append(db_heads[dup_of].split(";")[0] + "dup;tax=" + db_heads[dup_of].split("tax=")[1].replace("s:", "s:Dup"))
+    db_seqs.append(db_seqs[dup_of])
+    long_head = db_heads[long_of].split(";")[0] + "long;tax=" + db_heads[long_of].split("tax=")[1].replace("s:", "s:Long")
+    db_heads.insert(0, long_head)
+    db_seqs.insert(0, db_seqs[long_of] + b"A")
+    # shifted by the insertion: original long_of is now long_of + 1, dup_of + 1 and the duplicate is the last one
+    meta = {"tie_seqno": (dup_of + 1, len(db_seqs) - 1), "tie_length": (0, long_of + 1),
+            "lc_species": sorted(i + 1 for i in lc)}
+    db_heads.append("short;tax=d:Short;")
+    db_seqs.append(b"ACGTACGTACGTACGTACGT")   # 20 nt: dropped by --sintax (minseqlength 32)
+
+    q_heads, q_seqs = [], []
+
+    def window(s: bytes, up=True):
+        p = int(rng.integers(0, max(1, len(s) - q_len)))
+        w = s[p:p + q_len].upper() if up else s[p:p + q_len]
+        return mutate(rng, np.frombuffer(w, dtype=np.uint8), 0.03).tobytes()
+
+    sources = list(range(len(leaves))) + [dup_of] * 6 + [long_of] * 6
+    for i in range(n_q):
+        kind = i % 10
+        if kind == 9:
+            seq = random_seqs(rng, 1, q_len)[0].tobytes()
+        elif kind == 8:
+            seq = window(held[int(rng.integers(0, len(held)))][1].tobytes())
+        else:
+            src = sources[int(rng.integers(0, len(sources)))] if kind < 6 else sorted(lc)[i % len(lc)]
+            s = db_seqs[src + 1] if src != dup_of else db_seqs[dup_of + 1]
+            if kind >= 6:   # low-complexity region of an lc species, in upper case
+                lo = s.find(s[[c.islower() for c in s.decode()].index(True):][:20]) if any(chr(c).islower() for c in s) else 0
+                seq = s[max(0, lo - 40):max(0, lo - 40) + q_len].upper()
+            else:
+                seq = window(s)
+        if rng.random() < 0.3:
+            seq = revcomp(seq)
+        q_seqs.append(seq)
+        q_heads.append(f"q{i}" if i % 7 else f"q{i} sample=s{i % 5};")
+    # specials: fewer than 32 distinct k-mers, IUPAC / lower case, longer than 2 100 nt
+    specials = [("q_short10", b"ACGTTGCAAC"), ("q_short30", db_seqs[12][100:130]), ("q_polyA", b"A" * 120),
+                ("q_iupac", window(db_seqs[20])[:100] + b"NNRYKM" + window(db_seqs[20])[:120]),
+                ("q_lower", window(db_seqs[30]).lower()),
+                ("q_long1", db_seqs[40].upper() + db_seqs[41].upper()), ("q_long2", revcomp(db_seqs[50].upper() * 2))]
+    for j, (h, s) in enumerate(specials):
+        q_heads.insert(5 + 11 * j, h)
+        q_seqs.insert(5 + 11 * j, s)
+    meta["short_queries"] = [q_heads.index("q_short10"), q_heads.index("q_short30"), q_heads.index("q_polyA")]
+    meta["long_queries"] = [q_heads.index("q_long1"), q_heads.index("q_long2")]
+    return {"db_heads": db_heads, "db_seqs": db_seqs, "q_heads": q_heads, "q_seqs": q_seqs, "meta": meta}
+
+
+def write_records(path: str, heads, seqs, width: int = 80) -> None:
+    """FASTA with the given headers, sequence lines wrapped at `width`"""
+    with open(path, "wb") as f:
+        for h, s in zip(heads, seqs):
+            f.write(b">" + (h if isinstance(h, bytes) else h.encode()) + b"\n")
+            for i in range(0, max(len(s), 1), width):
+                f.write(s[i:i + width] + b"\n")
