@@ -327,8 +327,12 @@ int vsg_allpairs(vsg_ctx * ctx, const vsg_seqset * set, int64_t row0, int64_t nr
  *      of the reverse complement (the "-" of --uc column 5), whose statistics and CIGAR are those of the reverse-complemented
  *      sequence against the centroid: vsg_align_pairs(ctx, rc, set, ...) with rc from vsg_seqset_revcomp.  A centroid is
  *      always its plus strand.  A pair deferred to the fallback callback reaches it as (sequence, strand, centroid).
- *      The both-strands query set costs 2 bytes of device memory per nucleotide of `set`.  work (optional, 2 x int64):
- *      pairs and DP cells handed to the aligner, both strands counted. ---- */
+ *      The both-strands query set costs 2 bytes of device memory per nucleotide of `set`.  Any maxaccepts / maxrejects
+ *      is offered, clamped as cluster() clamps them (0 or more than the set: the number of sequences,
+ *      core/cluster.cpp:1213-1235), so --maxaccepts 0 --maxrejects 0 clusters exhaustively.  Above
+ *      maxaccepts + maxrejects + 8 = 1024 every round's candidates are kept on the host: about 144 bytes per candidate of
+ *      the round's query strands (a hit record and a list entry).  work (optional, 2 x int64): pairs and DP cells handed
+ *      to the aligner, both strands counted. ---- */
 typedef struct vsg_cluster_result {
   int32_t cluster;
   int32_t centroid;
@@ -350,7 +354,8 @@ int vsg_cluster_fast(vsg_ctx * ctx, const vsg_seqset * set, const vsg_search_opt
  *      to must outlive it.  vsg_cluster_session_assign handles the sequences [start, start + count) in rounds of
  *      round_size (cluster_assign_batch: the caller's --threads; cluster_assign_single: count = round_size = 1);
  *      ranges must be ascending and contiguous (cluster.hpp:104-111), results[i] belongs to sequence start + i.
- *      A session fed the whole set in one call gives vsg_cluster_fast's results. ---- */
+ *      A session fed the whole set in one call gives vsg_cluster_fast's results.  It offers the same limits (any
+ *      maxaccepts / maxrejects, clamped as vsg_cluster_fast clamps them) at the same host memory per round. ---- */
 typedef struct vsg_cluster_session vsg_cluster_session;
 int vsg_cluster_session_create(vsg_ctx * ctx, const vsg_seqset * set, const vsg_search_opts * opts, vsg_cluster_session ** out);
 int vsg_cluster_session_assign(vsg_cluster_session * session, int64_t start, int64_t count, int round_size,

@@ -42,6 +42,18 @@ inline int search_limits(const vsg_search_opts & o, int64_t seqcount, const char
   return VSG_OK;
 }
 
+// True when search_onequery's candidate loop (searchcore.cpp:915-954) will examine every candidate a query strand has
+// left: after `finalized` of its ncand candidates, neither limit nor the loop's guard can be reached before the list
+// ends, because each hit examined adds one accept or one reject.  Then none of that work is speculative, and the whole
+// remaining list can be one group, aligned in one device call instead of eight candidates per round; the pairs aligned
+// and the decisions are those of the groups of eight.  The search and cluster drivers apply it to the unbounded
+// ranker's lists, where a query can have thousands of candidates.
+inline bool exhaustible(int64_t ncand, int64_t finalized, int64_t accepts, int64_t rejects, int64_t maxaccepts, int64_t maxrejects)
+{
+  int64_t const left = ncand - finalized;
+  return left > MAXDELAYED && accepts + left <= maxaccepts && rejects + left <= maxrejects && ncand <= maxaccepts + maxrejects - 1;
+}
+
 // The statistics an aligner call returns, one entry per pair: score, aligned, matches, mismatches, gaps, and four
 // trims (vsg_align_pairs).
 struct PairResults {

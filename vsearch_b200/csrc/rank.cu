@@ -837,16 +837,26 @@ static int rank_status(int32_t status, const char * caller)
   return VSG_EINVAL;
 }
 
-// Launches rank_kernel<INCR, MODE> on c's stream over queries [q0, q0 + nq) (nq >= 1) against the nshards shards at
-// d_shards, whose targets' lengths `targets` holds: two CTAs per SM at most, and HBM scratch when a query has more than
-// KMER_CAP windows.  timed: ev[4..5] around the launch, added to vsg_profile.rank_ms by rank_collect_time.
-template <bool INCR, int MODE>
-static int rank_launch(vsg_ctx * c, const ShardDev * d_shards, int nshards, DevSeqs targets, int k, int mask_lower,
-                       const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches, int tophits,
-                       const RankTop & out, const int64_t * d_key_off, uint64_t * d_keys, bool timed)
+RankTargets index_targets(const vsg_index * ix, int mask_lower)
+{
+  RankTargets t;
+  t.shards = static_cast<const ShardDev *>(ix->b_shards.p); t.nshards = static_cast<int>(ix->h_shards.size());
+  t.lens = ix->db->d; t.k = ix->k; t.mask_lower = mask_lower; t.device = ix->device;
+  t.incr = false; t.timed = true;
+  return t;
+}
+
+// Launches rank_kernel<t.incr, MODE> on c's stream over queries [q0, q0 + nq) (nq >= 1) against t's shards: two CTAs per
+// SM at most, and HBM scratch when a query has more than KMER_CAP windows.  t.timed: ev[4..5] around the launch, added
+// to vsg_profile.rank_ms by rank_collect_time.
+template <int MODE>
+static int rank_launch(vsg_ctx * c, const RankTargets & t, const vsg_seqset * queries, int64_t q0, int64_t nq,
+                       int minwordmatches, int tophits, const RankTop & out, const int64_t * d_key_off, uint64_t * d_keys)
 {
   int rc;
-  VSG_CUDA_OK(cudaFuncSetAttribute(rank_kernel<INCR, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(RANK_SMEM)));
+  auto const kernel = t.incr ? rank_kernel<true, MODE> : rank_kernel<false, MODE>;
+  int const k = t.k;
+  VSG_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(RANK_SMEM)));
   int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
   int const grid = static_cast<int>(std::min<int64_t>(nq, static_cast<int64_t>(sms) * 2));
@@ -862,12 +872,12 @@ static int rank_launch(vsg_ctx * c, const ShardDev * d_shards, int nshards, DevS
     if ((rc = c->rank_scratch.reserve(sizeof(uint32_t) * stride * static_cast<size_t>(grid))) != VSG_OK) { return rc; }
     d_scratch = static_cast<uint32_t *>(c->rank_scratch.p);
   }
-  if (timed) { VSG_CUDA_OK(cudaEventRecord(c->ev[4], c->stream)); }
-  rank_kernel<INCR, MODE><<<grid, RANK_THREADS, RANK_SMEM, c->stream>>>(
-      queries->d, q0, static_cast<int>(nq), targets, d_shards, nshards, k, mask_lower, minwordmatches, tophits,
+  if (t.timed) { VSG_CUDA_OK(cudaEventRecord(c->ev[4], c->stream)); }
+  kernel<<<grid, RANK_THREADS, RANK_SMEM, c->stream>>>(
+      queries->d, q0, static_cast<int>(nq), t.lens, t.shards, t.nshards, k, t.mask_lower, minwordmatches, tophits,
       out.seqno, out.count, out.n, out.status, d_scratch, stride, bitmap_words, d_key_off, d_keys);
   count_launch();
-  if (timed) {
+  if (t.timed) {
     VSG_CUDA_OK(cudaEventRecord(c->ev[5], c->stream));
     c->rank_pending = true;
   }
@@ -884,9 +894,7 @@ int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, 
   if (nq > (1 << 30) / tophits) { Error::set("vsg_rank: batch too large"); return VSG_EINVAL; }
   int rc;
   if ((rc = rank_top_alloc(c, nq, tophits, out)) != VSG_OK || nq == 0) { return rc; }
-  return rank_launch<false, RANK_TOP>(c, static_cast<const ShardDev *>(ix->b_shards.p), static_cast<int>(ix->h_shards.size()),
-                                      ix->db->d, ix->k, mask_lower, queries, q0, nq, minwordmatches, tophits, out, nullptr,
-                                      nullptr, true);
+  return rank_launch<RANK_TOP>(c, index_targets(ix, mask_lower), queries, q0, nq, minwordmatches, tophits, out, nullptr, nullptr);
 }
 
 int rank_download(vsg_ctx * c, const RankTop & r, int64_t nq, int tophits, uint32_t * h_seqno, uint32_t * h_count,
@@ -920,20 +928,18 @@ __global__ void cut_lists_kernel(const uint64_t * __restrict__ keys, const int64
 
 // The count pass of the unbounded ranker: n[i] = the number of targets query q0 + i has at or above the reference's
 // threshold, min(minwordmatches, distinct k-mers) (its whole candidate list before any cut)
-int rank_counts(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
-                int mask_lower, std::vector<int32_t> & n)
+int rank_counts(vsg_ctx * c, const RankTargets & t, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                std::vector<int32_t> & n)
 {
   if (q0 < 0 || nq < 0 || q0 + nq > queries->d.n) { Error::set("vsg_rank: query range out of bounds"); return VSG_EINVAL; }
-  if (queries->device != c->device || ix->device != c->device) { Error::set("vsg_rank: sequence set / index lives on another device than the context"); return VSG_EINVAL; }
+  if (queries->device != c->device || t.device != c->device) { Error::set("vsg_rank: sequence set / index lives on another device than the context"); return VSG_EINVAL; }
   if (nq > (1 << 30)) { Error::set("vsg_rank: batch too large"); return VSG_EINVAL; }
   n.assign(static_cast<size_t>(nq), 0);
   if (nq == 0) { return VSG_OK; }
   RankTop r;
   int rc;
   if ((rc = rank_top_alloc(c, nq, 0, r)) != VSG_OK ||
-      (rc = rank_launch<false, RANK_COUNT>(c, static_cast<const ShardDev *>(ix->b_shards.p), static_cast<int>(ix->h_shards.size()),
-                                           ix->db->d, ix->k, mask_lower, queries, q0, nq, minwordmatches, 1, r, nullptr,
-                                           nullptr, true)) != VSG_OK) { return rc; }
+      (rc = rank_launch<RANK_COUNT>(c, t, queries, q0, nq, minwordmatches, 1, r, nullptr, nullptr)) != VSG_OK) { return rc; }
   int32_t status = 0;
   VSG_CUDA_OK(cudaMemcpyAsync(n.data(), r.n, sizeof(int32_t) * static_cast<size_t>(nq), cudaMemcpyDeviceToHost, c->stream));
   VSG_CUDA_OK(cudaMemcpyAsync(&status, r.status, sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
@@ -946,15 +952,15 @@ int rank_counts(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, i
 // targets with count >= min(minwordmatches, distinct k-mers) cut to tophits.  A count pass sizes every list; then, for
 // as many queries as the key budget holds at a time, an emit pass writes the keys, a segmented sort orders each
 // query's keys and cut_lists_kernel keeps the first tophits.  Keys, sort buffers and lists take 24 bytes per candidate
-// from a quarter of the context's direction-bit budget (a share of the device's free memory, vsg_ctx_create).  The
-// context's ranker time (vsg_profile.rank_ms) covers the count pass and, per chunk, the emit pass, sort and cut.
-int rank_lists(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
-               int64_t tophits, int mask_lower, std::vector<int64_t> & first, std::vector<uint32_t> & seqno,
-               std::vector<uint32_t> & count)
+// from a quarter of the context's direction-bit budget (a share of the device's free memory, vsg_ctx_create).  When
+// t.timed, the context's ranker time (vsg_profile.rank_ms) covers the count pass and, per chunk, the emit pass, sort and
+// cut.
+int rank_lists(vsg_ctx * c, const RankTargets & t, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+               int64_t tophits, std::vector<int64_t> & first, std::vector<uint32_t> & seqno, std::vector<uint32_t> & count)
 {
   if (tophits < 1) { Error::set("vsg_rank: tophits must be at least 1"); return VSG_EINVAL; }
   std::vector<int32_t> n;
-  int rc = rank_counts(c, ix, queries, q0, nq, minwordmatches, mask_lower, n);
+  int rc = rank_counts(c, t, queries, q0, nq, minwordmatches, n);
   if (rc != VSG_OK) { return rc; }
   first.assign(static_cast<size_t>(nq) + 1, 0);
   seqno.clear(); count.clear();
@@ -990,9 +996,7 @@ int rank_lists(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, in
       VSG_CUDA_OK(cudaMemcpyAsync(d_koff, koff.data(), sizeof(int64_t) * (static_cast<size_t>(m) + 1), cudaMemcpyHostToDevice, c->stream));
       VSG_CUDA_OK(cudaMemcpyAsync(d_ooff, ooff.data(), sizeof(int64_t) * (static_cast<size_t>(m) + 1), cudaMemcpyHostToDevice, c->stream));
       RankTop const emit{nullptr, nullptr, d_n2, d_n2 + m};
-      if ((rc = rank_launch<false, RANK_EMIT>(c, static_cast<const ShardDev *>(ix->b_shards.p), static_cast<int>(ix->h_shards.size()),
-                                              ix->db->d, ix->k, mask_lower, queries, q0 + a, m, minwordmatches, th, emit, d_koff,
-                                              d_k0, true)) != VSG_OK) { return rc; }
+      if ((rc = rank_launch<RANK_EMIT>(c, t, queries, q0 + a, m, minwordmatches, th, emit, d_koff, d_k0)) != VSG_OK) { return rc; }
       cub::DoubleBuffer<uint64_t> db(d_k0, d_k1);
       size_t tb = 0;
       cub::DeviceSegmentedSort::SortKeysDescending(nullptr, tb, db, static_cast<int>(keys), static_cast<int>(m), d_koff, d_koff + 1, c->stream);
@@ -1002,7 +1006,7 @@ int rank_lists(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, in
       if (nout > 0) {
         cut_lists_kernel<<<static_cast<unsigned>(m), 256, 0, c->stream>>>(db.Current(), d_koff, d_ooff, d_seq, d_cnt);
         count_launch();
-        VSG_CUDA_OK(cudaEventRecord(c->ev[5], c->stream));   // the chunk's ranker time runs from its emit pass to here
+        if (t.timed) { VSG_CUDA_OK(cudaEventRecord(c->ev[5], c->stream)); }   // the chunk's ranker time runs from its emit pass to here
         size_t const o = static_cast<size_t>(first[static_cast<size_t>(a)]);
         VSG_CUDA_OK(cudaMemcpyAsync(seqno.data() + o, d_seq, sizeof(uint32_t) * static_cast<size_t>(nout), cudaMemcpyDeviceToHost, c->stream));
         VSG_CUDA_OK(cudaMemcpyAsync(count.data() + o, d_cnt, sizeof(uint32_t) * static_cast<size_t>(nout), cudaMemcpyDeviceToHost, c->stream));
@@ -1030,7 +1034,7 @@ extern "C" int vsg_rank(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * qu
   if (tophits > TOPHITS_MAX) {
     std::vector<int64_t> first;
     std::vector<uint32_t> seqno, count;
-    int const rc = rank_lists(c, ix, queries, q0, nq, minwordmatches, tophits, mask_lower, first, seqno, count);
+    int const rc = rank_lists(c, index_targets(ix, mask_lower), queries, q0, nq, minwordmatches, tophits, first, seqno, count);
     if (rc != VSG_OK) { return rc; }
     for (int64_t i = 0; i < nq; i++) {
       size_t const a = static_cast<size_t>(first[static_cast<size_t>(i)]), n = static_cast<size_t>(first[static_cast<size_t>(i) + 1]) - a;
@@ -1190,19 +1194,16 @@ int cindex_append(vsg_ctx * c, CIndex * ix, const uint32_t * seqnos, int n)
 
 const std::vector<uint32_t> & cindex_seqnos(const CIndex * ix) { return ix->h_seqno; }
 
-// search_topscores of queries [q0, q0+nq) of `queries` against the targets added so far; results as rank_enqueue's,
-// candidate numbers are DENSE target numbers (CIndex::h_seqno maps them back).  Not timed.
-int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
-                        int tophits, RankTop & out)
+// The ranker's view of the targets added so far: their shard table, uploaded to ix->b_shards, and their lengths by
+// dense number.  Not timed.  t.nshards == 0 (nothing uploaded) while nothing is indexed.
+static int cindex_targets(vsg_ctx * c, CIndex * ix, RankTargets & t)
 {
-  if (tophits < 1 || tophits > TOPHITS_MAX) { Error::set("cluster ranker: tophits must be in 1..1024"); return VSG_EINVAL; }
-  int rc;
-  if ((rc = rank_top_alloc(c, nq, tophits, out)) != VSG_OK || nq == 0) { return rc; }
   int const nshards = static_cast<int>((ix->ncent + SHARD - 1) / SHARD);
-  if (nshards == 0) {   // nothing indexed yet: no candidates
-    VSG_CUDA_OK(cudaMemsetAsync(out.n, 0, sizeof(int32_t) * nq, c->stream));
-    return VSG_OK;
-  }
+  t.shards = nullptr; t.nshards = nshards;
+  t.lens = DevSeqs{nullptr, nullptr, static_cast<const int32_t *>(ix->b_clen.p), ix->ncent};
+  t.k = ix->k; t.mask_lower = ix->mask_lower; t.device = ix->device;
+  t.incr = true; t.timed = false;
+  if (nshards == 0) { return VSG_OK; }
   std::vector<ShardDev> sh(static_cast<size_t>(nshards));
   for (int s = 0; s < nshards; s++) {
     ShardDev & sd = sh[static_cast<size_t>(s)];
@@ -1213,12 +1214,45 @@ int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, in
     sd.t0 = s * SHARD;
     sd.nt = static_cast<int32_t>(std::min<int64_t>(SHARD, ix->ncent - static_cast<int64_t>(s) * SHARD));
   }
+  int rc;
   if ((rc = ix->b_shards.reserve(sizeof(ShardDev) * sh.size())) != VSG_OK) { return rc; }
   // pageable source: staged before the call returns, so `sh` may go out of scope
   VSG_CUDA_OK(cudaMemcpyAsync(ix->b_shards.p, sh.data(), sizeof(ShardDev) * sh.size(), cudaMemcpyHostToDevice, c->stream));
-  DevSeqs const lens{nullptr, nullptr, static_cast<const int32_t *>(ix->b_clen.p), ix->ncent};   // target lengths by dense number
-  return rank_launch<true, RANK_TOP>(c, static_cast<const ShardDev *>(ix->b_shards.p), nshards, lens, ix->k, ix->mask_lower,
-                                     queries, q0, nq, minwordmatches, tophits, out, nullptr, nullptr, false);
+  t.shards = static_cast<const ShardDev *>(ix->b_shards.p);
+  return VSG_OK;
+}
+
+// search_topscores of queries [q0, q0+nq) of `queries` against the targets added so far; results as rank_enqueue's,
+// candidate numbers are DENSE target numbers (CIndex::h_seqno maps them back).  Not timed.
+int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                        int tophits, RankTop & out)
+{
+  if (tophits < 1 || tophits > TOPHITS_MAX) { Error::set("cluster ranker: tophits must be in 1..1024"); return VSG_EINVAL; }
+  int rc;
+  if ((rc = rank_top_alloc(c, nq, tophits, out)) != VSG_OK || nq == 0) { return rc; }
+  RankTargets t;
+  if ((rc = cindex_targets(c, ix, t)) != VSG_OK) { return rc; }
+  if (t.nshards == 0) {   // nothing indexed yet: no candidates
+    VSG_CUDA_OK(cudaMemsetAsync(out.n, 0, sizeof(int32_t) * nq, c->stream));
+    return VSG_OK;
+  }
+  return rank_launch<RANK_TOP>(c, t, queries, q0, nq, minwordmatches, tophits, out, nullptr, nullptr);
+}
+
+// rank_lists of queries [q0, q0+nq) of `queries` against the targets added so far (any tophits); candidate numbers are
+// DENSE target numbers.  Not timed.
+int cindex_rank_lists(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                      int64_t tophits, std::vector<int64_t> & first, std::vector<uint32_t> & seqno, std::vector<uint32_t> & count)
+{
+  RankTargets t;
+  int const rc = cindex_targets(c, ix, t);
+  if (rc != VSG_OK) { return rc; }
+  if (t.nshards == 0) {   // nothing indexed yet: no candidates
+    first.assign(static_cast<size_t>(nq) + 1, 0);
+    seqno.clear(); count.clear();
+    return VSG_OK;
+  }
+  return rank_lists(c, t, queries, q0, nq, minwordmatches, tophits, first, seqno, count);
 }
 
 }  // namespace vsg

@@ -123,6 +123,19 @@ int index_wordlength(const vsg_index * ix);
 // the index's shards on its device (rank_steps.cuh)
 struct ShardDev;
 const ShardDev * index_shards(const vsg_index * ix, int & nshards);
+
+// What the ranker ranks against: a shard table on the device, the targets' lengths (only lens.len is read) and the
+// query-side masking.  incr: the cluster driver's incremental index (rank_kernel<true, MODE>), whose candidates are
+// dense target numbers.  timed: launches go into vsg_profile.rank_ms (the static index; the cluster ranker is untimed).
+struct RankTargets {
+  const ShardDev * shards = nullptr;
+  int nshards = 0;
+  DevSeqs lens{};
+  int k = 0, mask_lower = 0, device = 0;
+  bool incr = false, timed = false;
+};
+// the static index's targets, ranked with the query-side masking mask_lower
+RankTargets index_targets(const vsg_index * ix, int mask_lower);
 // enqueues the ranker over queries [q0, q0 + nq) on c's stream, timed into vsg_profile.rank_ms
 int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
                  int minwordmatches, int tophits, int mask_lower, RankTop & out);
@@ -130,12 +143,11 @@ int rank_enqueue(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, 
 int rank_download(vsg_ctx * c, const RankTop & r, int64_t nq, int tophits, uint32_t * h_seqno, uint32_t * h_count,
                   int32_t * h_n, const char * caller);
 // unbounded ranker (any tophits): query i's list is seqno / count[first[i] .. first[i + 1])
-int rank_lists(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
-               int64_t tophits, int mask_lower, std::vector<int64_t> & first, std::vector<uint32_t> & seqno,
-               std::vector<uint32_t> & count);
+int rank_lists(vsg_ctx * c, const RankTargets & t, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+               int64_t tophits, std::vector<int64_t> & first, std::vector<uint32_t> & seqno, std::vector<uint32_t> & count);
 // n[i] = how many targets query q0 + i has at or above the reference's threshold
-int rank_counts(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
-                int mask_lower, std::vector<int32_t> & n);
+int rank_counts(vsg_ctx * c, const RankTargets & t, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                std::vector<int32_t> & n);
 
 // the cluster driver's incremental index of the centroids; candidates are DENSE target numbers (cindex_seqnos maps
 // them to sequence numbers)
@@ -145,6 +157,9 @@ void cindex_destroy(CIndex * ix);
 int cindex_append(vsg_ctx * c, CIndex * ix, const uint32_t * seqnos, int n);
 int cindex_rank_enqueue(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
                         int tophits, RankTop & out);
+// rank_lists against the centroids indexed so far (tophits above RANK_TOPHITS_MAX); candidates are dense numbers
+int cindex_rank_lists(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int64_t q0, int64_t nq, int minwordmatches,
+                      int64_t tophits, std::vector<int64_t> & first, std::vector<uint32_t> & seqno, std::vector<uint32_t> & count);
 const std::vector<uint32_t> & cindex_seqnos(const CIndex * ix);
 
 // vsg_align_pairs with traceback on demand (align_ckpt.cuh, TbGate): leader_of[k] = index of pair k's group leader in
