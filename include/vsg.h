@@ -472,6 +472,37 @@ int vsg_sintax_rows(const vsg_sintax_result * results, int64_t nq, const char * 
 int vsg_sintax_stream(vsg_group * g, const char * const * target_headers, const char * query_fasta,
                       const vsg_sintax_opts * opts, int batch_queries, const char * tabbedout_path, vsg_stream_stats * stats);
 
+/* ---- read orientation: replaces the read loop of orient() (commands/orient.cpp:116-441) with unique_count
+ *      (core/unique.cpp:155-353), rc_kmer (orient.cpp:90-113) and Dbindex::getmatchcount.  vsg_orient decides for every
+ *      query of `queries` in [q0, q0 + nq), of any length, against an index made by vsg_index_create / vsg_udb_load: for
+ *      each DISTINCT k-mer w of the query at the index's word length (windows with a symbol outside ACGTU skipped, and with
+ *      a lower-case one iff query_mask_lower, i.e. --qmask other than none; the query is not DUST-masked), f = the
+ *      number of database sequences holding w and r = that of its reverse complement; count_fwd counts the w with
+ *      f > 8 r, count_rev those with r > 8 f.  strand 0 ('+') iff count_fwd >= 1 and count_fwd >= 4 count_rev, else
+ *      1 ('-') iff count_rev >= 1 and count_rev >= 4 count_fwd, else 2 ('?').  out[i] belongs to query q0 + i.  The first
+ *      call on an index builds its per-k-mer table of 4^k words in device memory (64 MiB at k = 12, 4 GiB at k = 15),
+ *      kept until vsg_index_destroy.  Device time goes into vsg_profile.rank_ms.
+ *      vsg_orient_stream is the --orient command over a FASTA or FASTQ file (the format from the first byte, '@' =
+ *      FASTQ; gzip / bzip2 files are refused): reader thread, vsg_orient on every device of the group, writer thread, all
+ *      outputs in input order.  fastaout / fastqout: '+' reads as read, '-' reads reverse-complemented (reverse_complement,
+ *      FASTQ qualities reversed); notmatched: '?' reads as read, in the input's format; tabbedout: "label\t+|-|?\tfwd\trev".
+ *      Labels are cut at the first blank unless notrunclabels; FASTA lines wrap at fasta_width (0: one line).  An output
+ *      path may be NULL (that output is off); all four NULL, or fastqout with FASTA input, is VSG_EINVAL, as are a FASTQ
+ *      record without its '@', a '+' line other than empty or the header, a file that ends inside a record and quality
+ *      that is not as long as the sequence (the message names the record).  nstrand (optional, 3 entries): the
+ *      reads oriented '+', '-' and '?'.  stats: `matched` counts the oriented reads, `rows` every read.  Header rewriting
+ *      (--relabel*, --sizeout, --xsize, --xee, --xlength, --lengthout, --label_suffix, --sample) is left to the
+ *      reference's writers. ---- */
+typedef struct vsg_orient_result {
+  int32_t strand;     /* 0 '+', 1 '-', 2 '?' */
+  uint32_t count_fwd, count_rev;
+} vsg_orient_result;
+int vsg_orient(vsg_ctx * ctx, const vsg_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
+               int query_mask_lower, vsg_orient_result * out);
+int vsg_orient_stream(vsg_group * g, const char * query_path, int query_mask_lower, int notrunclabels, int fasta_width,
+                      int batch_queries, const char * fastaout, const char * fastqout, const char * notmatched,
+                      const char * tabbedout, vsg_stream_stats * stats, int64_t * nstrand);
+
 #ifdef __cplusplus
 }
 #endif

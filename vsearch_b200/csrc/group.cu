@@ -275,6 +275,16 @@ int group_sintax(vsg_group * g, const char * qcat, const int64_t * qoff, const i
   });
 }
 
+int group_orient(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq, int query_mask_lower,
+                 vsg_orient_result * out)
+{
+  vsg_search_opts const none{};   // group_run's search options: no per-query arrays to rebase
+  return group_run(g, qcat, qoff, qlen, nq, 0, &none, nullptr,
+                   [&](int d, vsg_ctx * c, const vsg_seqset * q, int64_t b0, int64_t b1, const vsg_search_opts &, int64_t *) {
+    return vsg_orient(c, g->index[static_cast<size_t>(d)], q, 0, b1 - b0, query_mask_lower, out + b0);
+  });
+}
+
 }  // namespace vsg
 
 extern "C" int vsg_group_search_hits(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,

@@ -29,6 +29,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 
 namespace vsg {
 
@@ -86,6 +87,17 @@ __global__ void add_totals_kernel(const uint32_t * __restrict__ count /* 2 per k
 {
   size_t const i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i < hashsize) { totals[i] += count[2 * i] + count[2 * i + 1]; }
+}
+
+// the same totals from a built shard: sub-list i holds its k-mer's targets plus up to 7 POST_PAD entries (dense: k-mer
+// i >> 1; sparse: rkeys[i] >> 1)
+__global__ void shard_word_counts_kernel(ShardDev S, uint32_t nlists, uint32_t * __restrict__ totals)
+{
+  uint32_t const i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nlists) { return; }
+  uint32_t n = 0;
+  for (uint32_t j = S.start[i]; j < S.start[i + 1]; j++) { n += S.post[j] != POST_PAD ? 1u : 0u; }
+  if (n > 0) { atomicAdd(&totals[(S.nr != 0 ? S.rkeys[i] : i) >> 1], n); }
 }
 
 // ---- sparse build (--wordlength 11..15: 4^k list heads per shard would dwarf the postings) --------------------------
@@ -547,6 +559,11 @@ struct vsg_index {
   std::vector<ShardDev> h_shards;
   DevBuf b_shards;
   int64_t total_postings = 0;
+  // per k-mer, the number of targets holding it (Dbindex::getmatchcount), 4^k words: built on first use by
+  // index_word_counts, under the lock because an index is shared read-only by several contexts and threads
+  mutable std::mutex words_lock;
+  mutable DevBuf b_words;
+  mutable bool words_ready = false;
 };
 
 extern "C" void vsg_index_destroy(vsg_index * ix);
@@ -793,12 +810,35 @@ extern "C" void vsg_index_destroy(vsg_index * ix)
   for (auto & b : ix->b_post) { b.release(); }
   for (auto & b : ix->b_rkeys) { b.release(); }
   ix->b_shards.release();
+  ix->b_words.release();
   delete ix;
 }
 
 namespace vsg {
 const vsg_seqset * index_db(const vsg_index * ix) { return ix->db; }
 int index_wordlength(const vsg_index * ix) { return ix->k; }
+
+int index_word_counts(vsg_ctx * c, const vsg_index * ix, const uint32_t ** out)
+{
+  std::lock_guard<std::mutex> const lock(ix->words_lock);
+  if (!ix->words_ready) {
+    size_t const hashsize = static_cast<size_t>(1) << (2 * ix->k);
+    int const rc = ix->b_words.reserve(sizeof(uint32_t) * hashsize);
+    if (rc != VSG_OK) { return rc; }
+    uint32_t * const words = static_cast<uint32_t *>(ix->b_words.p);
+    VSG_CUDA_OK(cudaMemsetAsync(words, 0, sizeof(uint32_t) * hashsize, c->stream));
+    for (ShardDev const & S : ix->h_shards) {
+      uint32_t const nlists = S.nr != 0 ? S.nr : static_cast<uint32_t>(2 * hashsize);
+      shard_word_counts_kernel<<<(nlists + 255) / 256, 256, 0, c->stream>>>(S, nlists, words);
+      count_launch();
+    }
+    VSG_CUDA_OK(cudaStreamSynchronize(c->stream));
+    VSG_CUDA_OK(cudaGetLastError());
+    ix->words_ready = true;
+  }
+  *out = static_cast<const uint32_t *>(ix->b_words.p);
+  return VSG_OK;
+}
 const ShardDev * index_shards(const vsg_index * ix, int & nshards)
 {
   nshards = static_cast<int>(ix->h_shards.size());

@@ -1,4 +1,5 @@
-// stream.cu — the streaming --usearch_global driver (SURVEY.md §8 f1): FASTA in, --blast6out out.
+// stream.cu — the streaming command drivers (SURVEY.md §8 f1): --usearch_global (FASTA in, --blast6out out), --sintax
+// (--tabbedout out) and --orient (FASTA or FASTQ in, up to four outputs).
 //
 // Replaces, around vsg_group_search, the host loop of the reference's command
 //   search_thread_run / search_query      (commands/usearch_global.cpp:376-534)   read a query under mutex_input,
@@ -11,11 +12,13 @@
 // bottleneck; here parsing batch n+1 and formatting batch n-1 overlap the search of batch n.
 #include "vsg_internal.h"
 
+#include <algorithm>
 #include <chrono>
 #include <condition_variable>
 #include <cstdio>
 #include <cstring>
 #include <deque>
+#include <iterator>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -29,12 +32,15 @@ namespace {
 struct StreamBatch {
   int64_t first = 0;                 // index of the batch's first query in the file
   std::vector<char> cat;             // sequences back to back
+  std::vector<char> qual;            // FASTQ: the qualities at the sequences' offsets
+  bool fastq = false;
   std::vector<int64_t> off;
   std::vector<int32_t> len;
   std::vector<std::string> head;
   std::vector<vsg_search_result> res;   // query q's rows are res[row_first[q] .. row_first[q + 1])
   std::vector<int64_t> row_first;
   std::vector<vsg_sintax_result> tax;   // --sintax: one record per query
+  std::vector<vsg_orient_result> orient;   // --orient: one record per query
   bool last = false;
 };
 
@@ -79,21 +85,47 @@ double seconds_since(std::chrono::steady_clock::time_point t0)
   return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 
-// FASTA records of a file, one batch at a time (the reference's parser, core/fasta.cpp / fastx.cpp: a header runs
-// to the end of its line and is cut at the first blank unless --notrunclabels; sequence lines are joined, white
-// space dropped)
-class FastaReader {
+// FASTA or FASTQ records of a file, one batch at a time.  The format is that of the file's first byte, as fastx_open
+// finds it (core/fastx.cpp): '@' is FASTQ, anything else FASTA; gzip and bzip2 files are recognised by their magic bytes
+// and refused.  FASTA (core/fasta.cpp / fastx.cpp): a header runs to the end of its line and is cut at the first blank
+// unless --notrunclabels; sequence lines are joined, white space dropped.  FASTQ (core/fastq.cpp:324-581): a header line
+// that starts with '@', sequence lines up to the first line that starts with '+', a '+' line that is empty or repeats
+// the header, quality lines until the next line that starts with '@' once the quality is as long as the sequence; a
+// record that breaks one of these rules, ends early or has a quality of another length is an error.
+class FastxReader {
  public:
-  FastaReader(std::FILE * f, bool notrunc) : f_(f), notrunc_(notrunc), buf_(1 << 22) {}
+  enum Kind { FASTA, FASTQ, GZIP, BZIP2 };
+  FastxReader(std::FILE * f, bool notrunc) : f_(f), notrunc_(notrunc), buf_(1 << 22)
+  {
+    end_ = std::fread(buf_.data(), 1, buf_.size(), f_);
+    unsigned char const * const u = reinterpret_cast<unsigned char const *>(buf_.data());
+    if (end_ >= 2 && u[0] == 0x1f && u[1] == 0x8b) { kind_ = GZIP; }
+    else if (end_ >= 3 && u[0] == 'B' && u[1] == 'Z' && u[2] == 'h') { kind_ = BZIP2; }
+    else if (end_ >= 1 && u[0] == '@') { kind_ = FASTQ; }
+  }
+  Kind kind() const { return kind_; }
   // false when the file is exhausted and nothing was read
   bool fill(StreamBatch & b, int want, std::string & err)
   {
-    b.cat.clear(); b.off.clear(); b.len.clear(); b.head.clear();
+    b.cat.clear(); b.qual.clear(); b.off.clear(); b.len.clear(); b.head.clear();
+    b.fastq = kind_ == FASTQ;
+    if (kind_ == FASTQ) {
+      if (!fill_fastq(b, want, err)) { return false; }
+    } else {
+      fill_fasta(b, want, err);
+      if (!err.empty()) { return false; }
+    }
+    b.cat.push_back('\0');
+    return !b.head.empty();
+  }
+ private:
+  void fill_fasta(StreamBatch & b, int want, std::string & err)
+  {
     while (static_cast<int>(b.head.size()) < want) {
       if (!have_header_) {
         if (!next_line()) { break; }
         if (line_.empty()) { continue; }
-        if (line_[0] != '>') { err = "FASTA: a sequence line before the first header"; return false; }
+        if (line_[0] != '>') { err = "FASTA: a sequence line before the first header"; return; }
         pending_ = header_of(line_);
         have_header_ = true;
       }
@@ -105,15 +137,46 @@ class FastaReader {
         for (char ch : line_) { if (ch != ' ' && ch != '\t' && ch != '\r') { b.cat.push_back(ch); } }
       }
       int64_t const l = static_cast<int64_t>(b.cat.size()) - o;
-      if (l > 0x7fffffff) { err = "FASTA: a sequence longer than 2^31"; return false; }
+      if (l > 0x7fffffff) { err = "FASTA: a sequence longer than 2^31"; return; }
       b.off.push_back(o); b.len.push_back(static_cast<int32_t>(l)); b.head.push_back(pending_);
       if (more) { pending_ = header_of(line_); have_header_ = true; } else { have_header_ = false; }
       if (!more) { break; }
     }
-    b.cat.push_back('\0');
-    return !b.head.empty();
   }
- private:
+  bool fill_fastq(StreamBatch & b, int want, std::string & err)
+  {
+    while (static_cast<int>(b.head.size()) < want) {
+      if (!have_header_ && !next_line()) { break; }
+      have_header_ = false;
+      records_++;
+      auto fail = [&](const char * what) { err = "FASTQ record " + std::to_string(records_) + ": " + what; return false; };
+      if (line_.empty() || line_[0] != '@') { return fail("the header line does not start with '@'"); }
+      if (!newline_) { return fail("the file ends early"); }
+      header_line_.swap(line_);
+      b.head.push_back(header_of(header_line_));
+      int64_t const o = static_cast<int64_t>(b.cat.size());
+      for (;;) {
+        if (!next_line() || !newline_) { return fail("the file ends early"); }
+        if (!line_.empty() && line_[0] == '+') { break; }
+        b.cat.insert(b.cat.end(), line_.begin(), line_.end());
+      }
+      if (line_.size() > 1 && line_.compare(1, std::string::npos, header_line_, 1, std::string::npos) != 0) {
+        return fail("the '+' line is neither empty nor the header");
+      }
+      int64_t const l = static_cast<int64_t>(b.cat.size()) - o;
+      if (l > 0x7fffffff) { return fail("a sequence longer than 2^31"); }
+      bool first = true;
+      while (next_line()) {
+        if (!first && !line_.empty() && line_[0] == '@' && static_cast<int64_t>(b.qual.size()) - o == l) { have_header_ = true; break; }
+        first = false;
+        b.qual.insert(b.qual.end(), line_.begin(), line_.end());
+        if (static_cast<int64_t>(b.qual.size()) - o > l) { break; }
+      }
+      if (static_cast<int64_t>(b.qual.size()) - o != l) { return fail("the quality is not as long as the sequence"); }
+      b.off.push_back(o); b.len.push_back(static_cast<int32_t>(l));
+    }
+    return true;
+  }
   std::string header_of(const std::string & line) const
   {
     size_t e = line.size();
@@ -127,7 +190,7 @@ class FastaReader {
       if (pos_ == end_) {
         end_ = std::fread(buf_.data(), 1, buf_.size(), f_);
         pos_ = 0;
-        if (end_ == 0) { return !line_.empty() || got_partial_(); }
+        if (end_ == 0) { newline_ = false; return !line_.empty() || got_partial_(); }
       }
       char const * const s = buf_.data() + pos_;
       char const * const nl = static_cast<char const *>(std::memchr(s, '\n', end_ - pos_));
@@ -135,6 +198,7 @@ class FastaReader {
       line_.append(s, static_cast<size_t>(nl - s));
       pos_ += static_cast<size_t>(nl - s) + 1;
       partial_ = false;
+      newline_ = true;
       if (!line_.empty() && line_.back() == '\r') { line_.pop_back(); }
       return true;
     }
@@ -144,29 +208,47 @@ class FastaReader {
   bool notrunc_;
   std::vector<char> buf_;
   size_t pos_ = 0, end_ = 0;
-  bool partial_ = false;
-  std::string line_, pending_;
-  bool have_header_ = false;
+  bool partial_ = false, newline_ = false;   // newline_: the last line read ended with '\n'
+  Kind kind_ = FASTA;
+  int64_t records_ = 0;
+  std::string line_, pending_, header_line_;
+  bool have_header_ = false;   // line_ (FASTQ) or pending_ (FASTA) holds the next record's header
 };
 
-// The three stages over the batches of one FASTA file: the reader thread parses batches of batch_queries records,
-// the calling thread runs work(batch) (the GPU stage), the writer thread appends format(batch) to the output file in
-// input order.  Returns the first error of work, of the output file or of the parser, with `caller` in its message.
+// The three stages over the batches of one FASTA or FASTQ file: the reader thread parses batches of batch_queries
+// records, the calling thread runs work(batch) (the GPU stage), the writer thread has format(batch, outs, stats) fill
+// one string per output path and appends each to its file (a null path: no file) in input order.  need_fastq: FASTA
+// input is an error.  Returns the first error of work, of the output files or of the parser, with `caller` in its
+// message.
 template <class Work, class Format>
-int run_stream(const char * caller, const char * query_fasta, const char * out_path, bool notrunclabels, int batch_queries,
-               vsg_stream_stats * stats, Work && work, Format && format)
+int run_stream(const char * caller, const char * query_path, std::vector<const char *> const & out_paths, bool notrunclabels,
+               int batch_queries, bool need_fastq, vsg_stream_stats * stats, Work && work, Format && format)
 {
-  std::FILE * fin = std::fopen(query_fasta, "rb");
-  if (fin == nullptr) { Error::set(std::string(caller) + ": cannot open " + query_fasta); return VSG_EINVAL; }
-  std::FILE * fout = std::fopen(out_path, "wb");
-  if (fout == nullptr) { std::fclose(fin); Error::set(std::string(caller) + ": cannot write " + out_path); return VSG_EINVAL; }
+  std::FILE * fin = std::fopen(query_path, "rb");
+  if (fin == nullptr) { Error::set(std::string(caller) + ": cannot open " + query_path); return VSG_EINVAL; }
+  FastxReader fr(fin, notrunclabels);
+  char const * refused = nullptr;
+  if (fr.kind() == FastxReader::GZIP) { refused = ": gzip-compressed input is not supported: "; }
+  else if (fr.kind() == FastxReader::BZIP2) { refused = ": bzip2-compressed input is not supported: "; }
+  else if (need_fastq && fr.kind() != FastxReader::FASTQ) { refused = ": cannot write FASTQ output with FASTA input: "; }
+  if (refused != nullptr) { std::fclose(fin); Error::set(std::string(caller) + refused + query_path); return VSG_EINVAL; }
+  std::vector<std::FILE *> fout(out_paths.size(), nullptr);
+  for (size_t i = 0; i < out_paths.size(); i++) {
+    if (out_paths[i] == nullptr) { continue; }
+    fout[i] = std::fopen(out_paths[i], "wb");
+    if (fout[i] == nullptr) {
+      for (std::FILE * f : fout) { if (f != nullptr) { std::fclose(f); } }
+      std::fclose(fin);
+      Error::set(std::string(caller) + ": cannot write " + out_paths[i]);
+      return VSG_EINVAL;
+    }
+  }
 
   auto const t_wall = std::chrono::steady_clock::now();
   vsg_stream_stats st{};
   Channel parsed(2), searched(2);
   std::string reader_err;
   std::thread reader([&] {
-    FastaReader fr(fin, notrunclabels);
     int64_t first = 0;
     for (;;) {
       auto const t0 = std::chrono::steady_clock::now();
@@ -183,14 +265,16 @@ int run_stream(const char * caller, const char * query_fasta, const char * out_p
     parsed.put(std::move(e));
   });
   std::thread writer([&] {
-    std::string out;
+    std::vector<std::string> outs(out_paths.size());
     for (;;) {
       std::unique_ptr<StreamBatch> b = searched.get();
       if (b == nullptr || b->last) { break; }
       auto const t0 = std::chrono::steady_clock::now();
-      out.clear();
-      format(*b, out, st);
-      std::fwrite(out.data(), 1, out.size(), fout);
+      for (auto & o : outs) { o.clear(); }
+      format(*b, outs, st);
+      for (size_t i = 0; i < outs.size(); i++) {
+        if (fout[i] != nullptr) { std::fwrite(outs[i].data(), 1, outs[i].size(), fout[i]); }
+      }
       st.write_s += seconds_since(t0);
     }
   });
@@ -217,7 +301,9 @@ int run_stream(const char * caller, const char * query_fasta, const char * out_p
   reader.join();
   writer.join();
   std::fclose(fin);
-  if (std::fclose(fout) != 0 && rc == VSG_OK) { Error::set(std::string(caller) + ": write error"); rc = VSG_EINVAL; }
+  for (std::FILE * f : fout) {
+    if (f != nullptr && std::fclose(f) != 0 && rc == VSG_OK) { Error::set(std::string(caller) + ": write error"); rc = VSG_EINVAL; }
+  }
   if (rc == VSG_OK && !reader_err.empty()) { Error::set(std::string(caller) + ": " + reader_err); rc = VSG_EINVAL; }
   st.wall_s = seconds_since(t_wall);
   if (stats != nullptr) { *stats = st; }
@@ -236,12 +322,13 @@ extern "C" int vsg_usearch_stream(vsg_group * g, const char * const * target_lab
   }
   if (batch_queries < 1) { batch_queries = 65536; }
   if (maxhits < 0) { maxhits = 0; }
-  return run_stream("vsg_usearch_stream", query_fasta, blast6out_path, notrunclabels != 0, batch_queries, stats,
+  return run_stream("vsg_usearch_stream", query_fasta, {blast6out_path}, notrunclabels != 0, batch_queries, false, stats,
                     [&](StreamBatch & b) {
     // every row min(maxhits, hits) asks for, built on the host by the group search itself: no buffer to outgrow
     return group_search_rows(g, b.cat.data(), b.off.data(), b.len.data(), static_cast<int64_t>(b.head.size()), qmask_dust,
                              opts, maxhits, b.res, b.row_first, nullptr);
-  }, [&](StreamBatch const & b, std::string & out, vsg_stream_stats & st) {
+  }, [&](StreamBatch const & b, std::vector<std::string> & outs, vsg_stream_stats & st) {
+    std::string & out = outs[0];
     char row[256];
     size_t const nq = b.head.size();
     for (size_t q = 0; q < nq; q++) {
@@ -279,19 +366,109 @@ extern "C" int vsg_sintax_stream(vsg_group * g, const char * const * target_head
   int const rc = sintax_check_opts(opts, "vsg_sintax_stream");
   if (rc != VSG_OK) { return rc; }
   if (batch_queries < 1) { batch_queries = 65536; }
-  return run_stream("vsg_sintax_stream", query_fasta, tabbedout_path, true, batch_queries, stats, [&](StreamBatch & b) {
+  return run_stream("vsg_sintax_stream", query_fasta, {tabbedout_path}, true, batch_queries, false, stats, [&](StreamBatch & b) {
     vsg_sintax_opts o = *opts;
     o.query_number0 = b.first;
     b.tax.resize(b.head.size());
     return group_sintax(g, b.cat.data(), b.off.data(), b.len.data(), static_cast<int64_t>(b.head.size()), &o, b.tax.data());
-  }, [&](StreamBatch const & b, std::string & out, vsg_stream_stats & st) {
+  }, [&](StreamBatch const & b, std::vector<std::string> & outs, vsg_stream_stats & st) {
     std::vector<const char *> heads(b.head.size());
     for (size_t q = 0; q < heads.size(); q++) {
       heads[q] = b.head[q].c_str();
       vsg_sintax_result const & r = b.tax[q];
       if (r.nboot[r.strand] >= (VSG_SINTAX_BOOTSTRAPS + 1) / 2) { st.matched++; }
     }
-    sintax_rows_string(b.tax.data(), static_cast<int64_t>(heads.size()), heads.data(), target_headers, opts, out);
+    sintax_rows_string(b.tax.data(), static_cast<int64_t>(heads.size()), heads.data(), target_headers, opts, outs[0]);
     st.rows += static_cast<int64_t>(heads.size());
   });
+}
+
+namespace {
+
+// reverse_complement (utils/reverse_complement.cpp) with the reference's complement map (utils/maps.cpp): IUPAC codes
+// to their complements in the same case, U to A, anything else to N
+struct Complement {
+  char map[256];
+  Complement()
+  {
+    std::memset(map, 'N', sizeof map);
+    char const * const from = "ACGTURYKMBVDHSWNacgturykmbvdhswn";
+    char const * const to = "TGCAAYRMKVBHDSWNtgcaayrmkvbhdswn";
+    for (int i = 0; from[i] != '\0'; i++) { map[static_cast<unsigned char>(from[i])] = to[i]; }
+  }
+};
+
+// fasta_print_general / fasta_print_sequence (core/fasta.cpp:423-450, 482-...) without header rewriting: lines of
+// `width` symbols (width < 1: one line, also for an empty sequence)
+void fasta_record(std::string & out, const std::string & head, const char * seq, int64_t len, int width)
+{
+  out += '>'; out += head; out += '\n';
+  if (width < 1) { out.append(seq, static_cast<size_t>(len)); out += '\n'; return; }
+  for (int64_t i = 0; i < len; i += width) {
+    out.append(seq + i, static_cast<size_t>(std::min<int64_t>(width, len - i)));
+    out += '\n';
+  }
+}
+
+// fastq_print_general (core/fastq.cpp:681-785) without header rewriting
+void fastq_record(std::string & out, const std::string & head, const char * seq, const char * qual, int64_t len)
+{
+  out += '@'; out += head; out += '\n';
+  out.append(seq, static_cast<size_t>(len)); out += "\n+\n";
+  out.append(qual, static_cast<size_t>(len)); out += '\n';
+}
+
+}  // namespace
+
+// The --orient command (commands/orient.cpp:116-441) over the same pipeline; outs are fastaout, fastqout, notmatched,
+// tabbedout in that order.
+extern "C" int vsg_orient_stream(vsg_group * g, const char * query_path, int query_mask_lower, int notrunclabels, int fasta_width,
+                                 int batch_queries, const char * fastaout, const char * fastqout, const char * notmatched,
+                                 const char * tabbedout, vsg_stream_stats * stats, int64_t * nstrand)
+{
+  if (g == nullptr || query_path == nullptr) { Error::set("vsg_orient_stream: null argument"); return VSG_EINVAL; }
+  if (fastaout == nullptr && fastqout == nullptr && notmatched == nullptr && tabbedout == nullptr) {
+    Error::set("vsg_orient_stream: no output file (fastaout, fastqout, notmatched or tabbedout)");
+    return VSG_EINVAL;
+  }
+  if (batch_queries < 1) { batch_queries = 65536; }
+  static Complement const comp;
+  int64_t count[3] = {0, 0, 0};
+  int const rc = run_stream("vsg_orient_stream", query_path, {fastaout, fastqout, notmatched, tabbedout}, notrunclabels != 0,
+                            batch_queries, fastqout != nullptr, stats, [&](StreamBatch & b) {
+    b.orient.resize(b.head.size());
+    return group_orient(g, b.cat.data(), b.off.data(), b.len.data(), static_cast<int64_t>(b.head.size()), query_mask_lower,
+                        b.orient.data());
+  }, [&](StreamBatch const & b, std::vector<std::string> & outs, vsg_stream_stats & st) {
+    std::string rseq, rqual;
+    char row[64];
+    for (size_t q = 0; q < b.head.size(); q++) {
+      vsg_orient_result const & r = b.orient[q];
+      const char * seq = b.cat.data() + b.off[q];
+      const char * qual = b.fastq ? b.qual.data() + b.off[q] : nullptr;
+      int64_t const len = b.len[q];
+      count[r.strand]++;
+      if (r.strand == 1) {
+        rseq.resize(static_cast<size_t>(len));
+        for (int64_t i = 0; i < len; i++) { rseq[static_cast<size_t>(i)] = comp.map[static_cast<unsigned char>(seq[len - 1 - i])]; }
+        seq = rseq.data();
+        if (qual != nullptr) { rqual.assign(std::reverse_iterator<const char *>(qual + len), std::reverse_iterator<const char *>(qual)); qual = rqual.data(); }
+      }
+      if (r.strand != 2) {
+        st.matched++;
+        if (fastaout != nullptr) { fasta_record(outs[0], b.head[q], seq, len, fasta_width); }
+        if (fastqout != nullptr) { fastq_record(outs[1], b.head[q], seq, qual, len); }
+      } else if (notmatched != nullptr) {
+        if (b.fastq) { fastq_record(outs[2], b.head[q], seq, qual, len); } else { fasta_record(outs[2], b.head[q], seq, len, fasta_width); }
+      }
+      if (tabbedout != nullptr) {
+        int const w = std::snprintf(row, sizeof row, "\t%c\t%u\t%u\n", "+-?"[r.strand], r.count_fwd, r.count_rev);
+        outs[3] += b.head[q];
+        outs[3].append(row, static_cast<size_t>(w));
+      }
+      st.rows++;
+    }
+  });
+  if (nstrand != nullptr) { for (int s = 0; s < 3; s++) { nstrand[s] = count[s]; } }
+  return rc;
 }

@@ -123,6 +123,9 @@ int index_wordlength(const vsg_index * ix);
 // the index's shards on its device (rank_steps.cuh)
 struct ShardDev;
 const ShardDev * index_shards(const vsg_index * ix, int & nshards);
+// *out = the index's 4^k-word table on its device: per k-mer, the number of targets holding it (Dbindex::getmatchcount);
+// built from the shards with c's stream on the first call and kept until vsg_index_destroy
+int index_word_counts(vsg_ctx * c, const vsg_index * ix, const uint32_t ** out);
 
 // What the ranker ranks against: a shard table on the device, the targets' lengths (only lens.len is read) and the
 // query-side masking.  incr: the cluster driver's incremental index (rank_kernel<true, MODE>), whose candidates are
@@ -183,6 +186,9 @@ int group_search_rows(vsg_group * g, const char * qcat, const int64_t * qoff, co
 // vsg_sintax of host queries sharded over the group's devices; query i gets input number opts->query_number0 + i
 int group_sintax(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq,
                  const vsg_sintax_opts * opts, vsg_sintax_result * out);
+// vsg_orient of host queries sharded over the group's devices (group.cu)
+int group_orient(vsg_group * g, const char * qcat, const int64_t * qoff, const int32_t * qlen, int64_t nq, int query_mask_lower,
+                 vsg_orient_result * out);
 // VSG_EINVAL (message prefixed with caller) for --sintax_random or a cutoff outside 0..1 (sintax.cu)
 int sintax_check_opts(const vsg_sintax_opts * o, const char * caller);
 // the --tabbedout rows of vsg_sintax_rows, appended to `out` (sintax.cu)

@@ -332,6 +332,15 @@ class Context:
                                  res.ctypes.data_as(C.c_void_p) if nq > 0 else None), "vsg_sintax")
         return {k: res[k] for k in SINTAX_DT.names}
 
+    def orient(self, ix: IndexHandle, qs: SeqSetHandle, q0: int, nq: int, query_mask_lower: int = 1) -> np.ndarray:
+        """vsg_orient -> an (nq, 3) int64 array of (strand 0 '+' / 1 '-' / 2 '?', count_fwd, count_rev) for queries
+        q0 .. q0 + nq - 1"""
+        res = np.zeros(nq, dtype=ORIENT_DT)
+        _check(load().vsg_orient(self.h, ix.h, qs.h, C.c_int64(q0), C.c_int64(nq), C.c_int(query_mask_lower),
+                                 res.ctypes.data_as(C.c_void_p) if nq > 0 else None), "vsg_orient")
+        return np.stack([res["strand"].astype(np.int64), res["count_fwd"].astype(np.int64),
+                         res["count_rev"].astype(np.int64)], axis=1)
+
     def search(self, ix: IndexHandle, db: SeqSetHandle, qs: SeqSetHandle, q0: int, nq: int,
                opts: SearchOpts, max_results: int):
         res = (SearchResult * (nq * max_results))()
@@ -533,6 +542,23 @@ class Group:
         _check(load().vsg_sintax_stream(self.h, _strings(target_headers), query_fasta.encode(), C.byref(o), C.c_int(batch_queries),
                                         tabbedout.encode(), C.byref(st)), "vsg_sintax_stream")
         return {k: getattr(st, k) for k, _ in StreamStats._fields_}
+
+    def orient_stream(self, query_path: str, fastaout: Optional[str] = None, fastqout: Optional[str] = None,
+                      notmatched: Optional[str] = None, tabbedout: Optional[str] = None, query_mask_lower: int = 1,
+                      notrunclabels: int = 0, fasta_width: int = 80, batch_queries: int = 65536):
+        """vsg_orient_stream: the --orient command, FASTA or FASTQ file in, the given outputs out (None: off); returns
+        (statistics dict, (reads '+', '-', '?'))"""
+        st = StreamStats()
+        ns = np.zeros(3, dtype=np.int64)
+        enc = (lambda p: None if p is None else p.encode())
+        _check(load().vsg_orient_stream(self.h, query_path.encode(), C.c_int(query_mask_lower), C.c_int(notrunclabels),
+                                        C.c_int(fasta_width), C.c_int(batch_queries), enc(fastaout), enc(fastqout),
+                                        enc(notmatched), enc(tabbedout), C.byref(st), _ptr(ns, C.c_int64)),
+               "vsg_orient_stream")
+        return {k: getattr(st, k) for k, _ in StreamStats._fields_}, tuple(int(x) for x in ns)
+
+
+ORIENT_DT = np.dtype([("strand", np.int32), ("count_fwd", np.uint32), ("count_rev", np.uint32)])
 
 
 class SintaxOpts(C.Structure):

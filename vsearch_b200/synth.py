@@ -272,6 +272,97 @@ def sintax_data(seed: int = 77, length: int = 1450, fanout=(2, 2, 2, 2, 2, 2, 3)
     return {"db_heads": db_heads, "db_seqs": db_seqs, "q_heads": q_heads, "q_seqs": q_seqs, "meta": meta}
 
 
+def orient_data(seed: int = 91, n_roots: int = 40, per_root: int = 50, length: int = 1400, n_q: int = 360,
+                q_len: int = 250, long_len: int = 105_000):
+    """Reads of mixed orientation against a 16S-shaped database, for --orient.  The database: `n_roots` random roots of
+    ~`length` nt with `per_root` mutants each (4 %), so that a read's k-mers are held by many sequences; in one family
+    every other member is reverse-complemented (its k-mers are as common on both strands, so they vote for neither);
+    every 7th sequence has a random lower-case stretch of 120 nt and every 11th an upper-case low-complexity one of
+    100 nt (masking matters).  Reads (headers ``o{i}``, some with a blank and more text): mutated `q_len`-nt forward
+    windows, reverse-complemented windows, random reads, joins of a forward and a reverse-complemented window whose
+    shares fall on both sides of the 4x rule (either way round), reads shorter than 13 nt, reads with IUPAC codes and U,
+    reads with lower-case stretches, and one read of `long_len` nt made of database stretches.  FASTQ qualities are
+    random.  Returns dict(db_heads, db_seqs, q_heads, q_seqs, q_quals, meta)."""
+    rng = np.random.default_rng(seed)
+    db_heads, db_seqs = [], []
+    for r in range(n_roots):
+        root = random_seqs(rng, 1, length)[0]
+        for j in range(per_root):
+            s = mutate(rng, root, 0.04).tobytes()
+            i = len(db_seqs)
+            if i % 7 == 3:
+                p = int(rng.integers(50, len(s) - 200))
+                s = s[:p] + s[p:p + 120].lower() + s[p + 120:]
+            if i % 11 == 5:
+                unit = bytes(ACGT[rng.integers(0, 4, size=int(rng.integers(1, 4)))])
+                p = int(rng.integers(50, len(s) - 200))
+                s = s[:p] + (unit * 100)[:100] + s[p + 100:]
+            if r == 1 and j % 2 == 1:
+                s = revcomp(s)
+            db_seqs.append(s)
+            db_heads.append(f"db{i};root={r}")
+
+    def window(n, mut=0.03):
+        src = db_seqs[int(rng.integers(0, len(db_seqs)))].upper()
+        p = int(rng.integers(0, max(1, len(src) - n)))
+        return mutate(rng, np.frombuffer(src[p:p + n], dtype=np.uint8), mut).tobytes()
+
+    q_heads, q_seqs = [], []
+    kinds = []
+    for i in range(n_q):
+        kind = i % 9
+        if kind in (0, 1):
+            s = window(q_len)
+        elif kind in (2, 3):
+            s = revcomp(window(q_len))
+        elif kind == 4:
+            s = random_seqs(rng, 1, q_len)[0].tobytes()
+        elif kind in (5, 6):   # a forward and a reverse-complemented window, forward share around 4/5 (or 1/5)
+            share = float(rng.choice([0.5, 0.7, 0.76, 0.78, 0.8, 0.82, 0.84, 0.9, 0.95]))
+            a = int(round(2 * q_len * share))
+            s = window(a) + revcomp(window(2 * q_len - a))
+            if kind == 6:
+                s = revcomp(s)
+        elif kind == 7:        # IUPAC codes and U
+            s = bytearray(window(q_len))
+            for p in rng.integers(0, len(s), size=int(rng.integers(1, 12))):
+                s[int(p)] = b"NRYKMSWBDHVU"[int(rng.integers(0, 12))]
+            s = bytes(s)
+        else:                  # lower-case stretches
+            s = window(q_len)
+            if rng.random() < 0.5:
+                s = revcomp(s)
+            p = int(rng.integers(0, q_len - 60))
+            n = int(rng.integers(20, 200))
+            s = s[:p] + s[p:p + n].lower() + s[p + n:]
+        kinds.append(kind)
+        q_seqs.append(s)
+        q_heads.append(f"o{i}" if i % 5 else f"o{i} extra=text {kind}")
+    # reads shorter than the word length, and one of more than 100 000 nt from database stretches (a fifth of them
+    # reverse-complemented)
+    specials = [("o_short5", window(5)), ("o_short11", window(11)), ("o_short12", window(12)), ("o_short13", window(13))]
+    parts, n = [], 0
+    while n < long_len:
+        w = window(int(rng.integers(500, 1300)), 0.02)
+        parts.append(revcomp(w) if rng.random() < 0.2 else w)
+        n += len(parts[-1])
+    specials.append(("o_long", b"".join(parts)))
+    for j, (h, s) in enumerate(specials):
+        q_heads.insert(7 + 53 * j, h)
+        q_seqs.insert(7 + 53 * j, s)
+    q_quals = [bytes(rng.integers(33, 74, size=len(s), dtype=np.uint8)) for s in q_seqs]
+    meta = {"long_query": q_heads.index("o_long"),
+            "short_queries": [q_heads.index(h) for h in ("o_short5", "o_short11")]}
+    return {"db_heads": db_heads, "db_seqs": db_seqs, "q_heads": q_heads, "q_seqs": q_seqs, "q_quals": q_quals, "meta": meta}
+
+
+def write_fastq(path: str, heads, seqs, quals) -> None:
+    """FASTQ, one line per sequence and quality"""
+    with open(path, "wb") as f:
+        for h, s, q in zip(heads, seqs, quals):
+            f.write(b"@" + (h if isinstance(h, bytes) else h.encode()) + b"\n" + s + b"\n+\n" + q + b"\n")
+
+
 def write_records(path: str, heads, seqs, width: int = 80) -> None:
     """FASTA with the given headers, sequence lines wrapped at `width`"""
     with open(path, "wb") as f:
