@@ -1,5 +1,5 @@
 """The --orient parity cases shared by test_orient_cpu.py and test_orient_gpu.py: the synthetic reads and database
-(synth.orient_data), the option sets (a)-(g), their input files, a numpy restatement of the vote, and the reference
+(synth.orient_data), the option sets (a)-(i), their input files, a numpy restatement of the vote, and the reference
 CLI's results, stored in tests/golden/orient_reference.json under a name and a hash of the inputs (as
 sintax_cases.reference keys its records).  A record holds the digest of every output file, the (strand, count_fwd,
 count_rev) rows of --tabbedout and the three summary counts; for the --dbmask dust cases also the DUST mask of the
@@ -43,12 +43,79 @@ CASES = {
                    outs=("fastaout", "notmatched", "tabbedout"), opts=[]),
     "g_width0_notrunc": dict(k=12, dbmask="dust", qmask="dust", hardmask=False, fastq=False, udb=False, width=0, notrunc=True,
                              outs=("fastaout", "notmatched", "tabbedout"), opts=["--fasta_width", "0", "--notrunclabels"]),
+    # the small and the large end of the dense index.  At k = 4 every k-mer of data()'s database is about as common as its
+    # reverse complement, so h_k4 pins only the outcome "no read is oriented" (and the output files); the votes at
+    # k = 3..6 are pinned on biased_data() by biased_reference below
+    "h_k4": dict(k=4, dbmask="dust", qmask="dust", hardmask=False, fastq=False, udb=False, width=80, notrunc=False,
+                 outs=("fastaout", "notmatched", "tabbedout"), opts=["--wordlength", "4"]),
+    "i_k10": dict(k=10, dbmask="dust", qmask="dust", hardmask=False, fastq=False, udb=False, width=80, notrunc=False,
+                  outs=("fastaout", "notmatched", "tabbedout"), opts=["--wordlength", "10"]),
 }
 
 
 @functools.lru_cache(maxsize=None)
 def data():
     return synth.orient_data()
+
+
+@functools.lru_cache(maxsize=None)
+def biased_data():
+    """A database whose k-mers are strand-biased at every word length, so that reads are oriented even at k = 3..6: 300
+    targets of 60 nt drawn 45 % A, 45 % C, 5 % G, 5 % T (an A/C-rich k-mer is common, its G/T-rich reverse complement
+    rare), every 7th with a lower-case stretch and every 11th with an N.  Reads: mutated 40-nt windows of the targets on
+    either strand, joins of a forward and a reverse-complemented window, A/C-rich and uniform random reads, reads with a
+    lower-case stretch, and two reads shorter than 3 nt.  Returns dict(db (a (300, 60) ASCII matrix), db_heads, db_seqs,
+    q_heads, q_seqs)."""
+    rng = np.random.default_rng(97)
+    m = synth.ACGT[rng.choice(4, size=(300, 60), p=[0.45, 0.45, 0.05, 0.05])]
+    m[::7, 20:35] += ord("a") - ord("A")
+    m[3::11, 30] = ord("N")
+
+    def window():
+        s = m[int(rng.integers(0, 300))]
+        a = int(rng.integers(0, 21))
+        return synth.mutate(rng, s[a:a + 40], 0.02).tobytes()
+    q = []
+    for i in range(150):
+        kind = i % 6
+        if kind in (0, 1):
+            q.append(window())
+        elif kind == 2:
+            q.append(synth.revcomp(window()))
+        elif kind == 3:
+            a, b = window(), synth.revcomp(window())
+            q.append(a[:24] + b[:16] if i % 12 == 3 else b[:24] + a[:16])
+        elif kind == 4:
+            r = synth.ACGT[rng.choice(4, size=40, p=[0.45, 0.45, 0.05, 0.05])].tobytes()
+            q.append(synth.revcomp(r) if i % 12 == 4 else r)
+        else:
+            r = bytearray(synth.random_seqs(rng, 1, 40)[0].tobytes() if i % 12 == 5 else window())
+            r[10:25] = bytes(r[10:25]).lower()
+            q.append(bytes(r))
+    q += [b"AC", b"A"]
+    return dict(db=m, db_heads=[f"b{i}" for i in range(300)], db_seqs=[r.tobytes() for r in m],
+                q_heads=[f"q{i}" for i in range(len(q))], q_seqs=q)
+
+
+def run_biased_cli(k, mask, tmp):
+    """(reference CLI) the --tabbedout rows of `vsearch --orient` on biased_data() with --dbmask and --qmask `mask`"""
+    d = biased_data()
+    dbf, qf, tab = os.path.join(tmp, "bdb.fa"), os.path.join(tmp, "bq.fa"), os.path.join(tmp, "b.tsv")
+    synth.write_records(dbf, d["db_heads"], d["db_seqs"])
+    synth.write_records(qf, d["q_heads"], d["q_seqs"])
+    p = subprocess.run([checkers.STOCK, "--orient", qf, "--db", dbf, "--threads", "1", "--wordlength", str(k),
+                        "--dbmask", mask, "--qmask", mask, "--tabbedout", tab, "--quiet"],
+                       capture_output=True, text=True, timeout=600)
+    assert p.returncode == 0, p.stderr[-2000:]
+    return parse_rows(open(tab, "rb").read())
+
+
+def biased_reference(k, mask, compute=None):
+    """the stored rows of run_biased_cli(k, mask)"""
+    d = biased_data()
+    h = hashlib.sha256()
+    checkers._feed(h, [k, mask, d["db_heads"], d["db_seqs"], d["q_heads"], d["q_seqs"]])
+    return _record(f"orient_biased:k{k}_{mask}:{h.hexdigest()[:24]}", compute)
 
 
 def write_inputs(tmp):
@@ -146,10 +213,13 @@ _stored = None
 def reference(case, compute=None):
     """the stored reference record of `case`; VSG_RECORD_REFERENCE=1 with the compiled reference present recomputes it
     (compute()) and writes it to tests/golden/orient_reference.json"""
-    global _stored
     h = hashlib.sha256()
     checkers._feed(h, _inputs(case))
-    key = f"orient:{case}:{h.hexdigest()[:24]}"
+    return _record(f"orient:{case}:{h.hexdigest()[:24]}", compute)
+
+
+def _record(key, compute):
+    global _stored
     if os.environ.get("VSG_RECORD_REFERENCE") and reference_available() and compute is not None:
         val = compute()
         rec = json.load(open(GOLDEN)) if os.path.exists(GOLDEN) else {}

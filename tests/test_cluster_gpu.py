@@ -44,34 +44,35 @@ def _uc_records(text):
     return rec
 
 
-@pytest.mark.parametrize("threads,n,nroots,ident", [(1, 1500, 40, 0.97), (2, 1500, 40, 0.97), (8, 4000, 120, 0.97),
-                                                     (64, 6000, 400, 0.97), (16, 3000, 60, 0.90), (128, 30000, 150, 0.97)])
-def test_cluster_fast_equals_reference_cli(tmp_path, threads, n, nroots, ident):
-    seqs = _reads(n, nroots, seed=100 + threads)
-    labels = [f"a{i:07d}" for i in range(n)]
-    fa = str(tmp_path / "reads.fasta")
+def reference_records(tmp, name, key, seqs, labels, args):
+    """`vsearch --cluster_fast <reads> <args> --uc` on the reads (stored under `name` and `key`): (number of clusters,
+    digest of the S/H records)"""
+    fa = os.path.join(tmp, "reads.fasta")
     with open(fa, "wb") as f:
         for l, s in zip(labels, seqs):
             f.write(b">" + l.encode() + b"\n" + s + b"\n")
-    uc = str(tmp_path / "ref.uc")
+    uc = os.path.join(tmp, "ref.uc")
 
     def reduce(text):
         rec = _uc_records(text)
         return sum(1 for v in rec.values() if v[0] == "S"), checkers.digest(sorted(rec.items()))
-    nclusters, want = checkers.reference(
-        "cluster_fast", (seqs, labels, ident, threads),
-        lambda: checkers.run_stock(["--cluster_fast", fa, "--id", str(ident), "--threads", str(threads), "--uc", uc, "--quiet"],
-                                   [uc], reduce), os.path.exists(STOCK))
+    return checkers.reference(name, key, lambda: checkers.run_stock(["--cluster_fast", fa] + args + ["--uc", uc, "--quiet"],
+                                                                    [uc], reduce), os.path.exists(STOCK))
+
+
+def device_records(seqs, labels, ident, threads, wordlength=8):
+    """vsg_cluster_fast with the reference's --cluster_fast defaults: (number of clusters, digest of the S/H records
+    the reference would write, work)"""
+    n = len(seqs)
     # Database::sortbylength (core/db.cpp:433-449): length descending, abundance descending, label ascending, input order
     order = sorted(range(n), key=lambda i: (-len(seqs[i]), labels[i]))
     ss_host = synth.SeqSet([seqs[i] for i in order])
     ctx = vlib.Context(0)
     ss = ctx.seqset(ss_host)
     ss.dust()                                   # --qmask dust, the default (dust_all before clustering)
-    o = vlib.default_search_opts(); o.id = ident; o.mask_lower = 1
+    o = vlib.default_search_opts(); o.id = ident; o.mask_lower = 1; o.wordlength = wordlength
     o.maxrejects = 8                            # the reference's default for --cluster_fast (cli.cc:4163-4172); 32 elsewhere
     res, ncl, work = vlib.cluster_fast(ctx, ss, o, threads)
-    assert ncl == nclusters
     hq = [k for k in range(n) if res["centroid"][k] >= 0]
     al = ctx.align_pairs(ss, ss, np.array(hq, dtype=np.uint32), res["centroid"][hq].astype(np.uint32), cigar=True)
     cig = dict(zip(hq, al.cigars))
@@ -84,6 +85,18 @@ def test_cluster_fast_equals_reference_cli(tmp_path, threads, n, nroots, ident):
             c = cig[k]
             got[lab] = ("H", int(res["cluster"][k]), f"{res['id'][k]:.1f}", labels[order[int(res['centroid'][k])]],
                         "=" if res["id"][k] == 100.0 else c)   # '=' = identical ignoring terminal gaps (core/results.cpp:84-90)
-    assert checkers.digest(sorted(got.items())) == want
-    assert work[0] > 0 and work[1] > 0
     ss.close(); ctx.close()
+    return ncl, checkers.digest(sorted(got.items())), work
+
+
+@pytest.mark.parametrize("threads,n,nroots,ident", [(1, 1500, 40, 0.97), (2, 1500, 40, 0.97), (8, 4000, 120, 0.97),
+                                                     (64, 6000, 400, 0.97), (16, 3000, 60, 0.90), (128, 30000, 150, 0.97)])
+def test_cluster_fast_equals_reference_cli(tmp_path, threads, n, nroots, ident):
+    seqs = _reads(n, nroots, seed=100 + threads)
+    labels = [f"a{i:07d}" for i in range(n)]
+    nclusters, want = reference_records(str(tmp_path), "cluster_fast", (seqs, labels, ident, threads), seqs, labels,
+                                        ["--id", str(ident), "--threads", str(threads)])
+    ncl, got, work = device_records(seqs, labels, ident, threads)
+    assert ncl == nclusters
+    assert got == want
+    assert work[0] > 0 and work[1] > 0

@@ -1,5 +1,8 @@
 """Pins the oracle (oracle/*.c) against the UNMODIFIED reference compiled into
 oracle/_ref/libvsref.so, through the reference's stored results (checkers.reference).  CPU only."""
+import ctypes as C
+import re
+
 import numpy as np
 import pytest
 
@@ -196,3 +199,90 @@ def test_large_wordlengths_match_reference(k):
     _check_oracle(o, opts, qs, tops, rows)
     assert sum(len(o.topscores(q, opts)[0]) > 0 for q in qs) >= 25
     o.close()
+
+
+@pytest.mark.parametrize("k", [3, 4, 5, 6, 7, 9, 12])
+def test_other_wordlengths_match_reference(k):
+    """the word lengths the device tests trust the oracle at: with few targets the reference keeps most k-mers of small
+    k as bitmaps and counts them with its saturating SIMD path, the oracle with plain lists; candidate lists, whole
+    searches and the distinct k-mers of soft-masked and IUPAC queries still equal the reference's"""
+    rng = np.random.default_rng(200 + k)
+    db, roots = _family_db(rng)
+    o = _libs.OracleDb(db, k=k)
+    opts = _libs.search_opts(len(db), id=0.9, maxaccepts=2, maxrejects=16, k=k)
+    qs = [synth.mutate(rng, roots[i % roots.shape[0]], 0.05).tobytes()[: int(rng.integers(60, 300))] for i in range(30)]
+    qs += [b"ACGTACGTAC", synth.random_seqs(rng, 1, 200)[0].tobytes(), roots[0].tobytes()[:120] + b"NNRY" + roots[0].tobytes()[124:200],
+           roots[1].tobytes()[:100] + roots[1].tobytes()[100:200].lower(), roots[2].tobytes()[:k]]
+    th, tops, rows = _reference_search(db, qs, dict(k=k, id=0.9, maxaccepts=2, maxrejects=16))
+    assert opts.tophits == th
+    want = _libs.reference("unique_kmers_wordlength", (qs, k), lambda: _libs.digest(
+        [_libs.ref_unique_kmers(q, k, m) for q in qs for m in (0, 1)]), _libs.ref() is not None)
+    assert _libs.digest([_libs.oracle_unique_kmers(q, k, m) for q in qs for m in (0, 1)]) == want, k
+    _check_oracle(o, opts, qs, tops, rows)
+    assert sum(len(o.topscores(q, opts)[0]) > 0 for q in qs) >= 25
+    o.close()
+    # mask_lower = 1: the reference soft-masks its database by DUST (--dbmask dust, which upper-cases a sequence before
+    # lower-casing its low-complexity stretches) and leaves lower case out of the index and of the queries' k-mers.  Its
+    # search_topscores takes a query as given (the soft-masked one included); its search DUST-masks the query first.  The
+    # oracle gets the same sequences
+    masked = _libs.reference("dust_masked", ([db.seq(i) for i in range(len(db))], qs), lambda: [
+        [[m.start(), m.end()] for m in re.finditer(rb"[a-z]+", _dust(s))] for s in [db.seq(i) for i in range(len(db))] + qs],
+        _libs.ref() is not None)
+    dusted = [_apply_mask(s, iv) for s, iv in zip([db.seq(i) for i in range(len(db))] + qs, masked)]
+    assert sum(bool(iv) for iv in masked[:len(db)]) >= 2   # the low-complexity junk targets
+    dbm, qsm = synth.SeqSet(dusted[:len(db)]), dusted[len(db):]
+    th, tops, rows = _reference_search(db, qs, dict(k=k, id=0.9, maxaccepts=2, maxrejects=16, dust=1))
+    o = _libs.OracleDb(dbm, k=k, mask_lower=1)
+    opts = _libs.search_opts(len(db), id=0.9, maxaccepts=2, maxrejects=16, k=k, mask_lower=1)
+    assert _libs.digest([o.topscores(q, opts) for q in qs]) == tops
+    got = [[(h.target, h.id, h.matches, h.mismatches, h.nwgaps, h.nwalignmentlength, h.accepted, h.strand)
+            for h in o.search(q, opts)[0]] for q in qsm]
+    assert _libs.digest(got) == rows
+    o.close()
+
+
+def _dust(s: bytes) -> bytes:
+    """(reference) DUST soft-masking of one sequence"""
+    buf = C.create_string_buffer(s, len(s) + 1)
+    _libs.ref().vsref_dust(buf, C.c_int(len(s)))
+    return buf.raw[:len(s)]
+
+
+def _apply_mask(s: bytes, intervals) -> bytes:
+    """s upper-cased, with the [start, end) intervals lower-cased"""
+    b = bytearray(s.upper())
+    for a, e in intervals:
+        b[a:e] = bytes(b[a:e]).lower()
+    return bytes(b)
+
+
+@pytest.mark.parametrize("k", [10, 12])
+def test_count_cap_matches_reference(k):
+    """a 40 000-nt query with more than 32 767 distinct k-mers against copies of itself: the reference's counters
+    saturate at 32 767 (searchcore.cpp:306-315) and so do the oracle's; length, then seqno, orders the saturated copies"""
+    rng = np.random.default_rng(300 + k)
+    q = synth.random_seqs(rng, 1, 40_000)[0]
+    seqs = [s.tobytes() for s in synth.random_seqs(rng, 60, 200)]
+    seqs[7] = seqs[30] = q.tobytes()
+    seqs[3] = q.tobytes() + b"A"
+    seqs[2] = b"GT" + q.tobytes()
+    seqs[40] = np.concatenate([q[:20_000], synth.mutate(rng, q[20_000:], 0.3)]).tobytes()
+    db = synth.SeqSet(seqs)
+    qs = [q.tobytes(), q[:5000].tobytes()]
+
+    def run_reference():
+        r = _libs.RefDb(db, k=k, id=0.9, maxaccepts=2, maxrejects=16)
+        tops = [r.topscores(x) for x in qs]
+        th = r.tophits
+        r.close()
+        return th, _libs.digest(tops), _libs.digest([_libs.ref_unique_kmers(x, k) for x in qs])
+    th, tops, kmers = _libs.reference("count_cap_topscores", (db, qs, k), run_reference, _libs.ref() is not None)
+    opts = _libs.search_opts(len(db), id=0.9, maxaccepts=2, maxrejects=16, k=k)
+    assert opts.tophits == th
+    assert _libs.digest([_libs.oracle_unique_kmers(x, k) for x in qs]) == kmers
+    assert _libs.oracle_unique_kmers(qs[0], k).shape[0] > 32767
+    o = _libs.OracleDb(db, k=k)
+    got = [o.topscores(x, opts) for x in qs]
+    o.close()
+    assert _libs.digest(got) == tops
+    assert got[0][0][:5].tolist() == [7, 30, 3, 2, 40] and got[0][1][:4].tolist() == [32767] * 4 and got[0][1][4] < 32767

@@ -28,6 +28,19 @@ def test_restatement_matches_reference_rows(case, tmp_path):
     assert [int((s == v).sum()) for v in range(3)] == rec["summary"]
 
 
+@pytest.mark.parametrize("k", [3, 4, 5, 6])
+@pytest.mark.parametrize("mask", ["none", "soft"])
+def test_restatement_matches_reference_votes_at_short_wordlengths(k, mask, tmp_path):
+    """on the strand-biased fixture reads are oriented both ways even at k = 3..6, and the restatement's rows equal the
+    reference CLI's there too"""
+    d = oc.biased_data()
+    want = oc.biased_reference(k, mask, lambda: oc.run_biased_cli(k, mask, str(tmp_path)))
+    skip = mask == "soft"
+    assert oc.orient_rows(d["q_seqs"], k, skip, *oc.word_counts(d["db_seqs"], k, skip)) == want
+    r = np.array(want)
+    assert set(r[:, 0]) == {0, 1, 2} and (r[:, 1] > 0).sum() > 20 and (r[:, 2] > 0).sum() > 20, (k, mask)
+
+
 def test_fixture_covers_the_rules():
     """every case has reads of all three outcomes; the joins fall on both sides of the 4x rule; short reads get 0/0"""
     d = oc.data()
