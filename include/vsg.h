@@ -435,6 +435,47 @@ int vsg_udb_words(const vsg_udb * udb, const uint32_t ** kmercount, const uint32
 int vsg_udb_load(vsg_ctx * ctx, const vsg_udb * udb, vsg_seqset ** db, vsg_index ** index, int * mask_lower);
 int vsg_group_create_udb(const int * devices, int ndev, const vsg_scoring * scoring, const vsg_udb * udb, vsg_group ** out);
 
+/* ---- making UDB files: replaces makeudb_usearch (commands/makeudb_usearch.cpp:105-273) with Dbindex::prepare /
+ *      add_all_sequences (core/dbindex.cpp:121-255) built on the device.  vsg_udb_make makes, from n records as db.read
+ *      keeps them (any case; headers as they go into the file), the same in-memory database vsg_udb_open makes from a
+ *      file: the records upper-cased (db.read(..., upcase = 1)), with --dbmask dust DUST-masked on the device (masked
+ *      symbols lower case, or 'N' with hardmask), and the word index at `wordlength` built on the device: per word the
+ *      ascending numbers of the sequences holding it, from the windows without a masked symbol (outside ACGTU; with
+ *      --dbmask soft or dust also lower case).  Every accessor, vsg_udb_load and vsg_group_create_udb take the result.
+ *      The device scratch is bounded by a quarter of the context's direction-bit budget (VSG_DIR_BUDGET_MB), at most
+ *      1 GiB; the host holds kmercount[4^k] (4 GiB at k = 15) and the index.  The length limits of opts are not applied
+ *      here.  vsg_udb_write writes the file makeudb_usearch writes, byte for byte; a failed write removes the file.
+ *      vsg_makeudb_usearch is the --makeudb_usearch command: FASTA or FASTQ in (the format from the first byte; gzip and
+ *      bzip2 refused), labels cut at the first blank unless notrunclabels, db.read's symbol rules (FASTA: core/fasta.cpp's
+ *      table, other printable symbols stripped and counted, '.', '-' and control characters an error naming the line;
+ *      FASTQ: IUPAC letters only), records outside [minseqlength, maxseqlength] discarded and counted (minseqlength < 1:
+ *      no lower bound), then vsg_udb_make and vsg_udb_write.  A file is written even when every record is discarded
+ *      (the reference's own reader, and vsg_udb_open, refuse such a file).  Errors leave no output file. ---- */
+#define VSG_DBMASK_NONE 0
+#define VSG_DBMASK_SOFT 1
+#define VSG_DBMASK_DUST 2
+typedef struct vsg_makeudb_opts {
+  int32_t wordlength;     /* --wordlength, 3..15 (default 8) */
+  int32_t dbmask;         /* --dbmask: VSG_DBMASK_NONE / _SOFT / _DUST (default dust) */
+  int32_t hardmask;       /* --hardmask: DUST-masked symbols become 'N' (no effect with soft or none: the input is upper-cased) */
+  int32_t notrunclabels;  /* --notrunclabels */
+  int64_t minseqlength;   /* --minseqlength (default 32 for this command, cli.cc) */
+  int64_t maxseqlength;   /* --maxseqlength (default 50 000) */
+} vsg_makeudb_opts;
+void vsg_makeudb_opts_default(vsg_makeudb_opts * opts);
+typedef struct vsg_makeudb_stats {
+  int64_t sequences;          /* records kept */
+  int64_t discarded_short, discarded_long;
+  int64_t stripped;           /* FASTA symbols stripped with a warning by the reference (digits, '*', blanks, ...) */
+  int64_t nucleotides, index_entries;
+  double parse_s, device_s, write_s, wall_s;
+} vsg_makeudb_stats;
+int vsg_udb_make(vsg_ctx * ctx, const char * cat, const int64_t * off, const int32_t * len, const char * const * headers,
+                 int64_t n, const vsg_makeudb_opts * opts, vsg_udb ** out);
+int vsg_udb_write(const vsg_udb * udb, const char * path);
+int vsg_makeudb_usearch(vsg_ctx * ctx, const char * input_path, const vsg_makeudb_opts * opts, const char * output_path,
+                        vsg_makeudb_stats * stats);
+
 /* ---- SINTAX taxonomy classification: replaces sintax_query / sintax_search_topscores / sintax_analyse
  *      (commands/sintax.cpp:138-516) for --sintax with --randseed.  vsg_sintax runs the 100 bootstraps of every query
  *      of `queries` in [q0, q0 + nq) and of its reverse complement (strand_both) against an index made by

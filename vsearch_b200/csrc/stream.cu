@@ -85,6 +85,33 @@ double seconds_since(std::chrono::steady_clock::time_point t0)
   return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 
+// db.read's rules for the records it keeps (core/db.cpp, core/fasta.cpp, core/fastq.cpp), which only --makeudb_usearch
+// applies; the search, --sintax and --orient streams read with the default (no rules).
+//   symbols: FASTA sequence bytes by core/fasta.cpp's action table — the IUPAC letters kept, tab, VT, FF and CR dropped
+//            silently, other control bytes, '-' and '.' an error naming the line, anything else stripped and counted;
+//            control bytes in a header an error.  FASTQ sequence bytes: IUPAC letters only; quality bytes: 33..126.
+//   minlen / maxlen: records shorter or longer are discarded and counted.
+struct FastxRules {
+  bool symbols = false;
+  int64_t minlen = 0, maxlen = INT64_MAX;
+  int64_t stripped = 0, discarded_short = 0, discarded_long = 0;
+};
+
+enum class Sym : unsigned char { keep, strip, drop, reject, unprintable };
+
+bool iupac_letter(unsigned char ch)
+{
+  return ((ch >= 'A' && ch <= 'Z') || (ch >= 'a' && ch <= 'z')) && std::strchr("ABCDGHKMNRSTUVWY", ch & ~0x20) != nullptr;
+}
+
+Sym fasta_symbol(unsigned char ch)
+{
+  if (ch == '\t' || ch == 11 || ch == 12 || ch == '\r') { return Sym::drop; }
+  if (ch < 32) { return Sym::unprintable; }
+  if (ch == '-' || ch == '.') { return Sym::reject; }
+  return iupac_letter(ch) ? Sym::keep : Sym::strip;
+}
+
 // FASTA or FASTQ records of a file, one batch at a time.  The format is that of the file's first byte, as fastx_open
 // finds it (core/fastx.cpp): '@' is FASTQ, anything else FASTA; gzip and bzip2 files are recognised by their magic bytes
 // and refused.  FASTA (core/fasta.cpp / fastx.cpp): a header runs to the end of its line and is cut at the first blank
@@ -95,7 +122,7 @@ double seconds_since(std::chrono::steady_clock::time_point t0)
 class FastxReader {
  public:
   enum Kind { FASTA, FASTQ, GZIP, BZIP2 };
-  FastxReader(std::FILE * f, bool notrunc) : f_(f), notrunc_(notrunc), buf_(1 << 22)
+  FastxReader(std::FILE * f, bool notrunc, FastxRules * rules = nullptr) : f_(f), notrunc_(notrunc), rules_(rules), buf_(1 << 22)
   {
     end_ = std::fread(buf_.data(), 1, buf_.size(), f_);
     unsigned char const * const u = reinterpret_cast<unsigned char const *>(buf_.data());
@@ -128,18 +155,28 @@ class FastxReader {
         if (line_[0] != '>') { err = "FASTA: a sequence line before the first header"; return; }
         pending_ = header_of(line_);
         have_header_ = true;
+        if (!check_header(pending_, err)) { return; }
       }
       // sequence lines up to the next header
       int64_t const o = static_cast<int64_t>(b.cat.size());
       bool more = false;
       while (next_line()) {
         if (!line_.empty() && line_[0] == '>') { more = true; break; }
-        for (char ch : line_) { if (ch != ' ' && ch != '\t' && ch != '\r') { b.cat.push_back(ch); } }
+        if (rules_ != nullptr && rules_->symbols) {
+          if (!fasta_line(b, err)) { return; }
+        } else {
+          for (char ch : line_) { if (ch != ' ' && ch != '\t' && ch != '\r') { b.cat.push_back(ch); } }
+        }
       }
       int64_t const l = static_cast<int64_t>(b.cat.size()) - o;
       if (l > 0x7fffffff) { err = "FASTA: a sequence longer than 2^31"; return; }
-      b.off.push_back(o); b.len.push_back(static_cast<int32_t>(l)); b.head.push_back(pending_);
-      if (more) { pending_ = header_of(line_); have_header_ = true; } else { have_header_ = false; }
+      if (keep(b, o, l)) { b.off.push_back(o); b.len.push_back(static_cast<int32_t>(l)); b.head.push_back(pending_); }
+      if (more) {
+        pending_ = header_of(line_); have_header_ = true;
+        if (!check_header(pending_, err)) { return; }
+      } else {
+        have_header_ = false;
+      }
       if (!more) { break; }
     }
   }
@@ -153,12 +190,22 @@ class FastxReader {
       if (line_.empty() || line_[0] != '@') { return fail("the header line does not start with '@'"); }
       if (!newline_) { return fail("the file ends early"); }
       header_line_.swap(line_);
-      b.head.push_back(header_of(header_line_));
+      std::string head = header_of(header_line_);
+      if (!check_header(head, err)) { return false; }
       int64_t const o = static_cast<int64_t>(b.cat.size());
+      bool const symbols = rules_ != nullptr && rules_->symbols;
       for (;;) {
         if (!next_line() || !newline_) { return fail("the file ends early"); }
         if (!line_.empty() && line_[0] == '+') { break; }
-        b.cat.insert(b.cat.end(), line_.begin(), line_.end());
+        if (symbols) {
+          for (char ch : line_) {
+            if (ch == '\r') { continue; }
+            if (!iupac_letter(static_cast<unsigned char>(ch))) { return fail(illegal("sequence", ch).c_str()); }
+            b.cat.push_back(ch);
+          }
+        } else {
+          b.cat.insert(b.cat.end(), line_.begin(), line_.end());
+        }
       }
       if (line_.size() > 1 && line_.compare(1, std::string::npos, header_line_, 1, std::string::npos) != 0) {
         return fail("the '+' line is neither empty nor the header");
@@ -169,13 +216,68 @@ class FastxReader {
       while (next_line()) {
         if (!first && !line_.empty() && line_[0] == '@' && static_cast<int64_t>(b.qual.size()) - o == l) { have_header_ = true; break; }
         first = false;
+        if (symbols) {
+          for (char ch : line_) {
+            if (ch < 33 || ch > 126) { return fail(illegal("quality", ch).c_str()); }
+          }
+        }
         b.qual.insert(b.qual.end(), line_.begin(), line_.end());
         if (static_cast<int64_t>(b.qual.size()) - o > l) { break; }
       }
       if (static_cast<int64_t>(b.qual.size()) - o != l) { return fail("the quality is not as long as the sequence"); }
-      b.off.push_back(o); b.len.push_back(static_cast<int32_t>(l));
+      if (keep(b, o, l)) { b.off.push_back(o); b.len.push_back(static_cast<int32_t>(l)); b.head.push_back(std::move(head)); }
+      else { b.qual.resize(static_cast<size_t>(o)); }
     }
     return true;
+  }
+  // the rules' length limits: false (the record's bytes removed, the discard counted) for a record outside them
+  bool keep(StreamBatch & b, int64_t o, int64_t l)
+  {
+    if (rules_ == nullptr) { return true; }
+    if (l >= rules_->minlen && l <= rules_->maxlen) { return true; }
+    (l < rules_->minlen ? rules_->discarded_short : rules_->discarded_long)++;
+    b.cat.resize(static_cast<size_t>(o));
+    return false;
+  }
+  // a FASTA sequence line under the rules' symbol table
+  bool fasta_line(StreamBatch & b, std::string & err)
+  {
+    for (char ch : line_) {
+      unsigned char const u = static_cast<unsigned char>(ch);
+      switch (fasta_symbol(u)) {
+        case Sym::keep: b.cat.push_back(ch); break;
+        case Sym::strip: rules_->stripped++; break;
+        case Sym::drop: break;
+        case Sym::reject:
+          err = std::string("Illegal character '") + ch + "' in sequence on line " + std::to_string(lineno_) + " of FASTA file";
+          return false;
+        case Sym::unprintable:
+          err = "Illegal unprintable ASCII character no " + std::to_string(u) + " in sequence on line " + std::to_string(lineno_) +
+                " of FASTA file";
+          return false;
+      }
+    }
+    return true;
+  }
+  // fastx_filter_header: no control byte but tab, no DEL, in the label as it is kept
+  bool check_header(const std::string & head, std::string & err) const
+  {
+    if (rules_ == nullptr || !rules_->symbols) { return true; }
+    for (char ch : head) {
+      unsigned char const u = static_cast<unsigned char>(ch);
+      if (u == 127 || (u > 0 && u < 32 && u != '\t')) {
+        err = "Illegal character encountered in FASTA/FASTQ header: unprintable ASCII character no " + std::to_string(u) +
+              " on line " + std::to_string(lineno_);
+        return false;
+      }
+    }
+    return true;
+  }
+  std::string illegal(const char * what, char ch) const
+  {
+    unsigned char const u = static_cast<unsigned char>(ch);
+    std::string const sym = (u > 32 && u < 127) ? std::string("'") + ch + "'" : "(unprintable, no " + std::to_string(u) + ")";
+    return std::string("Illegal ") + what + " character " + sym + " on line " + std::to_string(lineno_);
   }
   std::string header_of(const std::string & line) const
   {
@@ -190,7 +292,12 @@ class FastxReader {
       if (pos_ == end_) {
         end_ = std::fread(buf_.data(), 1, buf_.size(), f_);
         pos_ = 0;
-        if (end_ == 0) { newline_ = false; return !line_.empty() || got_partial_(); }
+        if (end_ == 0) {
+          newline_ = false;
+          bool const got = !line_.empty() || got_partial_();
+          lineno_ += got ? 1 : 0;
+          return got;
+        }
       }
       char const * const s = buf_.data() + pos_;
       char const * const nl = static_cast<char const *>(std::memchr(s, '\n', end_ - pos_));
@@ -199,6 +306,7 @@ class FastxReader {
       pos_ += static_cast<size_t>(nl - s) + 1;
       partial_ = false;
       newline_ = true;
+      lineno_++;
       if (!line_.empty() && line_.back() == '\r') { line_.pop_back(); }
       return true;
     }
@@ -206,11 +314,13 @@ class FastxReader {
   bool got_partial_() { bool const p = partial_; partial_ = false; return p; }
   std::FILE * f_;
   bool notrunc_;
+  FastxRules * rules_;
   std::vector<char> buf_;
   size_t pos_ = 0, end_ = 0;
   bool partial_ = false, newline_ = false;   // newline_: the last line read ended with '\n'
   Kind kind_ = FASTA;
   int64_t records_ = 0;
+  int64_t lineno_ = 0;   // the number of the line last read, from 1
   std::string line_, pending_, header_line_;
   bool have_header_ = false;   // line_ (FASTQ) or pending_ (FASTA) holds the next record's header
 };
@@ -471,4 +581,61 @@ extern "C" int vsg_orient_stream(vsg_group * g, const char * query_path, int que
   });
   if (nstrand != nullptr) { for (int s = 0; s < 3; s++) { nstrand[s] = count[s]; } }
   return rc;
+}
+
+// The --makeudb_usearch command (commands/makeudb_usearch.cpp:105-273): the whole file parsed under db.read's rules, the
+// database made on the device (vsg_udb_make), the file written (vsg_udb_write).  The stages run one after another: the
+// file's word index, which comes before its sequences, needs every sequence.
+extern "C" int vsg_makeudb_usearch(vsg_ctx * c, const char * input_path, const vsg_makeudb_opts * opts, const char * output_path,
+                                   vsg_makeudb_stats * stats)
+{
+  if (c == nullptr || input_path == nullptr || opts == nullptr) { Error::set("vsg_makeudb_usearch: null argument"); return VSG_EINVAL; }
+  if (output_path == nullptr) { Error::set("vsg_makeudb_usearch: UDB output file must be specified"); return VSG_EINVAL; }
+  int rc = makeudb_check_opts(opts, "vsg_makeudb_usearch");
+  if (rc != VSG_OK) { return rc; }
+  auto const t_wall = std::chrono::steady_clock::now();
+  vsg_makeudb_stats st{};
+  std::FILE * fin = std::fopen(input_path, "rb");
+  if (fin == nullptr) { Error::set(std::string("vsg_makeudb_usearch: cannot open ") + input_path); return VSG_EINVAL; }
+  FastxRules rules;
+  rules.symbols = true;
+  rules.minlen = std::max<int64_t>(opts->minseqlength, 0);
+  rules.maxlen = opts->maxseqlength;
+  StreamBatch b;
+  std::string err;
+  {
+    FastxReader fr(fin, opts->notrunclabels != 0, &rules);
+    if (fr.kind() == FastxReader::GZIP) { err = "gzip-compressed input is not supported"; }
+    else if (fr.kind() == FastxReader::BZIP2) { err = "bzip2-compressed input is not supported"; }
+    else { fr.fill(b, INT32_MAX, err); }
+  }
+  std::fclose(fin);
+  if (!err.empty()) { Error::set(std::string("vsg_makeudb_usearch: ") + err + " (" + input_path + ")"); return VSG_EINVAL; }
+  if (b.cat.empty()) { b.cat.push_back('\0'); }
+  int64_t const n = static_cast<int64_t>(b.head.size());
+  std::vector<const char *> heads(static_cast<size_t>(n));
+  for (int64_t i = 0; i < n; i++) { heads[static_cast<size_t>(i)] = b.head[static_cast<size_t>(i)].c_str(); }
+  st.parse_s = seconds_since(t_wall);
+
+  auto const t_dev = std::chrono::steady_clock::now();
+  vsg_udb * u = nullptr;
+  rc = vsg_udb_make(c, b.cat.data(), b.off.data(), b.len.data(), heads.data(), n, opts, &u);
+  st.device_s = seconds_since(t_dev);
+  if (rc != VSG_OK) { return rc; }
+  auto const t_write = std::chrono::steady_clock::now();
+  rc = vsg_udb_write(u, output_path);
+  st.write_s = seconds_since(t_write);
+  vsg_udb_info info{};
+  vsg_udb_info_get(u, &info);
+  vsg_udb_close(u);
+  if (rc != VSG_OK) { return rc; }
+  st.sequences = n;
+  st.discarded_short = rules.discarded_short;
+  st.discarded_long = rules.discarded_long;
+  st.stripped = rules.stripped;
+  st.nucleotides = info.nucleotides;
+  st.index_entries = info.index_entries;
+  st.wall_s = seconds_since(t_wall);
+  if (stats != nullptr) { *stats = st; }
+  return VSG_OK;
 }

@@ -36,17 +36,6 @@ namespace vsg {
 int index_create_counts(vsg_ctx * c, const vsg_seqset * db, int wordlength, int mask_lower, uint32_t * d_totals, vsg_index ** out);
 }
 
-struct vsg_udb {
-  vsg_udb_info info{};
-  std::vector<uint32_t> kmercount;   // 4^k
-  std::vector<uint32_t> kmerindex;   // info.index_entries
-  std::vector<char> headers;         // header block (NUL-terminated strings)
-  std::vector<uint32_t> header_off;  // seqcount + 1
-  std::vector<char> cat;             // sequences back to back, one NUL at the very end
-  std::vector<int64_t> off;
-  std::vector<int32_t> len;
-};
-
 namespace {
 
 constexpr uint32_t UDB_MAGIC = 0x55444246u;   // "FBDU" on disk, udb.cpp:127

@@ -199,6 +199,9 @@ int sintax_rows_string(const vsg_sintax_result * res, int64_t nq, const char * c
 int hits_out(const std::vector<vsg_search_result> & rows, const std::vector<int64_t> & first, const char * caller,
              vsg_search_result * hits, int64_t cap, int64_t * first_out, int64_t * nhits);
 
+// VSG_EINVAL (message prefixed with caller) for a word length outside 3..15 or an unknown dbmask (makeudb.cu)
+int makeudb_check_opts(const vsg_makeudb_opts * o, const char * caller);
+
 // owning handle of a sequence set
 struct SeqsetDeleter { void operator()(vsg_seqset * s) const { vsg_seqset_destroy(s); } };
 using SeqsetPtr = std::unique_ptr<vsg_seqset, SeqsetDeleter>;
@@ -218,6 +221,18 @@ struct vsg_seqset {
   vsg::DevBuf b_sym, b_off, b_len;
   int device = 0;
   int64_t total = 0;
+};
+
+// a UDB database in host memory: read from a file (vsg_udb_open, udb.cu) or made from sequences (vsg_udb_make, makeudb.cu)
+struct vsg_udb {
+  vsg_udb_info info{};
+  std::vector<uint32_t> kmercount;   // 4^k
+  std::vector<uint32_t> kmerindex;   // info.index_entries
+  std::vector<char> headers;         // header block (NUL-terminated strings)
+  std::vector<uint32_t> header_off;  // seqcount + 1
+  std::vector<char> cat;             // sequences back to back, one NUL at the very end
+  std::vector<int64_t> off;
+  std::vector<int32_t> len;
 };
 
 struct vsg_ctx {

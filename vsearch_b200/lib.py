@@ -305,6 +305,29 @@ class Context:
                                        C.byref(h)), "vsg_index_create")
         return IndexHandle(h)
 
+    def udb_make(self, seqs, headers, wordlength=8, dbmask="dust", hardmask=False) -> "Udb":
+        """vsg_udb_make: the in-memory UDB database of the records `seqs` (bytes each) with `headers` (str each)"""
+        o = makeudb_opts(wordlength=wordlength, dbmask=dbmask, hardmask=hardmask)
+        cat = np.frombuffer(b"".join(seqs) + b"\0", dtype=np.uint8)
+        ln = np.array([len(x) for x in seqs], dtype=np.int32)
+        off = np.zeros(len(seqs), dtype=np.int64)
+        if len(seqs) > 1:
+            off[1:] = np.cumsum(ln[:-1], dtype=np.int64)
+        hs = (C.c_char_p * max(1, len(headers)))(*[h.encode() for h in headers])
+        h = C.c_void_p()
+        _check(load().vsg_udb_make(self.h, cat.ctypes.data_as(C.c_char_p), _ptr(off, C.c_int64), _ptr(ln, C.c_int32), hs,
+                                   C.c_int64(len(seqs)), C.byref(o), C.byref(h)), "vsg_udb_make")
+        return Udb._wrap(h)
+
+    def makeudb_usearch(self, input_path: str, output_path: Optional[str], **opts) -> dict:
+        """vsg_makeudb_usearch (the --makeudb_usearch command); opts as makeudb_opts; returns the stats as a dict"""
+        o = makeudb_opts(**opts)
+        st = MakeudbStats()
+        _check(load().vsg_makeudb_usearch(self.h, input_path.encode(), C.byref(o),
+                                          output_path.encode() if output_path is not None else None, C.byref(st)),
+               "vsg_makeudb_usearch")
+        return {k: getattr(st, k) for k, _ in MakeudbStats._fields_}
+
     def udb_load(self, udb: "Udb"):
         """vsg_udb_load: (SeqSetHandle, IndexHandle, mask_lower) of a parsed UDB file"""
         sh = C.c_void_p(); ih = C.c_void_p(); ml = C.c_int(-1)
@@ -612,14 +635,26 @@ def udb_detect(path: str) -> bool:
 
 
 class Udb:
-    """A parsed UDB file (host side; no GPU needed): vsg_udb_open and its accessors."""
+    """A parsed UDB file (host side; no GPU needed): vsg_udb_open and its accessors; or a database made by
+    Context.udb_make (vsg_udb_make)."""
 
-    def __init__(self, path: str):
+    def __init__(self, path: Optional[str], _handle=None):
         self.h = C.c_void_p()
-        _check(load().vsg_udb_open(path.encode(), C.byref(self.h)), "vsg_udb_open")
+        if _handle is not None:
+            self.h = _handle
+        else:
+            _check(load().vsg_udb_open(path.encode(), C.byref(self.h)), "vsg_udb_open")
         self.info = UdbInfo()
         _check(load().vsg_udb_info_get(self.h, C.byref(self.info)), "vsg_udb_info_get")
         self.n = int(self.info.sequences)
+
+    @classmethod
+    def _wrap(cls, handle) -> "Udb":
+        return cls(None, _handle=handle)
+
+    def write(self, path: str):
+        """vsg_udb_write: the file makeudb_usearch would write"""
+        _check(load().vsg_udb_write(self.h, path.encode()), "vsg_udb_write")
 
     def close(self):
         if self.h:
@@ -656,4 +691,29 @@ class StreamStats(C.Structure):
 def default_search_opts() -> SearchOpts:
     o = SearchOpts()
     load().vsg_search_opts_default(C.byref(o))
+    return o
+
+
+DBMASK = {"none": 0, "soft": 1, "dust": 2}
+
+
+class MakeudbOpts(C.Structure):
+    _fields_ = [("wordlength", C.c_int32), ("dbmask", C.c_int32), ("hardmask", C.c_int32), ("notrunclabels", C.c_int32),
+                ("minseqlength", C.c_int64), ("maxseqlength", C.c_int64)]
+
+
+class MakeudbStats(C.Structure):
+    _fields_ = [("sequences", C.c_int64), ("discarded_short", C.c_int64), ("discarded_long", C.c_int64),
+                ("stripped", C.c_int64), ("nucleotides", C.c_int64), ("index_entries", C.c_int64),
+                ("parse_s", C.c_double), ("device_s", C.c_double), ("write_s", C.c_double), ("wall_s", C.c_double)]
+
+
+def makeudb_opts(**kw) -> MakeudbOpts:
+    """vsg_makeudb_opts_default, then the given fields; dbmask may be "none" / "soft" / "dust" or the number"""
+    o = MakeudbOpts()
+    load().vsg_makeudb_opts_default(C.byref(o))
+    for k, v in kw.items():
+        if k == "dbmask" and isinstance(v, str):
+            v = DBMASK[v]
+        setattr(o, k, int(v))
     return o
