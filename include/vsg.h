@@ -544,6 +544,76 @@ int vsg_orient_stream(vsg_group * g, const char * query_path, int query_mask_low
                       int batch_queries, const char * fastaout, const char * fastqout, const char * notmatched,
                       const char * tabbedout, vsg_stream_stats * stats, int64_t * nstrand);
 
+/* ---- clustering commands: replaces cluster() (core/cluster.cpp:1140-1430), which --cluster_fast, --cluster_size,
+ *      --cluster_smallmem and --cluster_unoise all run (commands/cluster_{fast,size,smallmem,unoise}.cpp), for --uc,
+ *      --centroids and --clusters output.  vsg_cluster_command: the whole file read as db.read(..., upcase = 0) keeps it
+ *      (FASTA or FASTQ, the format from the first byte, gzip / bzip2 refused, labels cut at the first blank unless
+ *      notrunclabels, case kept), records outside [minseqlength, maxseqlength] and, for --cluster_unoise, of abundance
+ *      below minsize discarded and counted.  The abundance is always read from ";size=" (1 without it; zero or out of
+ *      range is an error, header_get_size) and orders the records, drives --sizeorder and the unoise rule; sizein only
+ *      decides whether the C records and --sizeout sum abundances or count members.  Sort on the host by command
+ *      (db.cpp:433-485): _FAST by length desc, abundance desc, label (strcmp) asc, input order; _SIZE and _UNOISE by
+ *      abundance desc, label asc, input order; _SMALLMEM keeps the input order, which must be length-descending unless
+ *      usersort.  Then on the device: the set made, masked (qmask dust: vsg_seqset_dust; soft: lower case out of the
+ *      words; soft + hardmask: lower case turned into 'N' first), clustered by vsg_cluster_fast with round_size =
+ *      threads (the results depend on it, as the reference's depend on --threads), target_sizes = the abundances and,
+ *      for --self, target_labels = label identities (the caller leaves those pointer fields of `s` NULL), unoise set
+ *      for _UNOISE; the CIGARs of the H records from two vsg_align_pairs calls (plus-strand members against the set,
+ *      minus-strand ones from a vsg_seqset_revcomp set).  The printed sequences have the input's letters and the
+ *      device's case (the DUST mask).  Then vsg_cluster_write.  Refused with VSG_EINVAL and no output file: compressed
+ *      input, --qmask dust --hardmask, a word length outside 3..10, an unsorted _SMALLMEM input without usersort, and a
+ *      pair the 16-bit aligner defers (its CIGAR cannot come from the fallback callback).  Not offered: --alnout,
+ *      --samout, --userout, --blast6out, --matched, --notmatched, OTU tables, --msaout, --consout, --profile,
+ *      --relabel_sha1 / _md5 / _self, --label_suffix, --sample, several GPUs.  The reference's stderr summary is `stats`.
+ *      vsg_cluster_cmd_opts_default fills each command's CLI defaults (cli.cc): maxrejects 8 for --cluster_fast and 32
+ *      otherwise, weak_id 0.90, minsize 8 and id -1 (not given) for --cluster_unoise, minseqlength 32, maxseqlength 50 000,
+ *      wordlength 8, qmask dust, fasta_width 80; the caller sets id and whatever else the user gave.
+ *      vsg_cluster_write needs no device: the output files of n records in processing (sorted) order — headers as kept,
+ *      sequences as printed (cat / off / len), abundances, the vsg_cluster_result of each and the CIGAR of each H record
+ *      (cigar_buf + cigar_off[i], NUL-terminated; ignored for S records).  --uc: S / H records in processing order
+ *      (results_show_uc_one; "=" when matches == the alignment length without terminal gaps for _FAST, == the
+ *      alignment length otherwise, results.cpp:84-95), then one C record per cluster; --centroids (fasta_print_general
+ *      with --sizeout, --xsize, --relabel, --clusterout_id, fasta_width); --clusters: file <prefix><cluster number> per
+ *      cluster.  C records, centroids and cluster files follow cluster number, or with clusterout_sort the cluster
+ *      abundance descending first.  Any path may be NULL (no such output).  A failed write removes every file the call
+ *      made.  *singletons (optional): clusters of abundance 1. ---- */
+#define VSG_CLUSTER_FAST 0
+#define VSG_CLUSTER_SIZE 1
+#define VSG_CLUSTER_SMALLMEM 2
+#define VSG_CLUSTER_UNOISE 3
+typedef struct vsg_cluster_cmd_opts {
+  int32_t command;          /* VSG_CLUSTER_FAST / _SIZE / _SMALLMEM / _UNOISE */
+  int32_t threads;          /* --threads: the round size of vsg_cluster_fast */
+  int32_t qmask;            /* --qmask: VSG_DBMASK_NONE / _SOFT / _DUST (default dust) */
+  int32_t hardmask;         /* --hardmask (with qmask soft: lower case becomes 'N'; refused with dust) */
+  int32_t usersort;         /* --usersort (_SMALLMEM: any input order) */
+  int32_t notrunclabels;    /* --notrunclabels */
+  int32_t sizein;           /* --sizein: C records and --sizeout sum the abundances instead of counting members */
+  int32_t sizeout;          /* --sizeout */
+  int32_t xsize;            /* --xsize: ";size=" stripped from printed labels */
+  int32_t clusterout_id;    /* --clusterout_id: ";clusterid=" on the centroids */
+  int32_t clusterout_sort;  /* --clusterout_sort */
+  int32_t fasta_width;      /* --fasta_width (default 80; 0: one line) */
+  int64_t minseqlength;     /* --minseqlength (default 32) */
+  int64_t maxseqlength;     /* --maxseqlength (default 50 000) */
+  int64_t minsize;          /* --minsize (_UNOISE only; default 8) */
+  const char * relabel;     /* --relabel prefix of the centroids and cluster files, or NULL */
+} vsg_cluster_cmd_opts;
+typedef struct vsg_cluster_cmd_stats {
+  int64_t sequences;        /* records kept */
+  int64_t discarded_short, discarded_long, discarded_minsize;
+  int64_t clusters, singletons, nucleotides;
+  int64_t pairs, cells;     /* vsg_cluster_fast's work */
+  double parse_s, sort_s, device_s, cigar_s, write_s, wall_s;
+} vsg_cluster_cmd_stats;
+void vsg_cluster_cmd_opts_default(int command, vsg_cluster_cmd_opts * c, vsg_search_opts * s);
+int vsg_cluster_command(vsg_ctx * ctx, const char * input_path, const vsg_cluster_cmd_opts * c, const vsg_search_opts * s,
+                        const char * uc, const char * centroids, const char * clusters_prefix, vsg_cluster_cmd_stats * stats);
+int vsg_cluster_write(int64_t n, const char * const * headers, const char * cat, const int64_t * off, const int32_t * len,
+                      const int64_t * abundances, const vsg_cluster_result * results, const char * cigar_buf,
+                      const int64_t * cigar_off, const vsg_cluster_cmd_opts * c, const char * uc, const char * centroids,
+                      const char * clusters_prefix, int64_t * singletons);
+
 #ifdef __cplusplus
 }
 #endif

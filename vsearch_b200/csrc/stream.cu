@@ -85,8 +85,8 @@ double seconds_since(std::chrono::steady_clock::time_point t0)
   return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 
-// db.read's rules for the records it keeps (core/db.cpp, core/fasta.cpp, core/fastq.cpp), which only --makeudb_usearch
-// applies; the search, --sintax and --orient streams read with the default (no rules).
+// db.read's rules for the records it keeps (core/db.cpp, core/fasta.cpp, core/fastq.cpp), which --makeudb_usearch and the
+// clustering commands apply (read_fastx_file); the search, --sintax and --orient streams read with the default (no rules).
 //   symbols: FASTA sequence bytes by core/fasta.cpp's action table — the IUPAC letters kept, tab, VT, FF and CR dropped
 //            silently, other control bytes, '-' and '.' an error naming the line, anything else stripped and counted;
 //            control bytes in a header an error.  FASTQ sequence bytes: IUPAC letters only; quality bytes: 33..126.
@@ -583,6 +583,37 @@ extern "C" int vsg_orient_stream(vsg_group * g, const char * query_path, int que
   return rc;
 }
 
+// The whole of a FASTA or FASTQ file under db.read's rules (FastxRules): the records --makeudb_usearch and the clustering
+// commands read into memory before they start.
+int vsg::read_fastx_file(const char * caller, const char * path, bool notrunclabels, int64_t minlen, int64_t maxlen, FastxFile & out)
+{
+  std::FILE * fin = std::fopen(path, "rb");
+  if (fin == nullptr) { Error::set(std::string(caller) + ": cannot open " + path); return VSG_EINVAL; }
+  FastxRules rules;
+  rules.symbols = true;
+  rules.minlen = std::max<int64_t>(minlen, 0);
+  rules.maxlen = maxlen;
+  StreamBatch b;
+  std::string err;
+  {
+    FastxReader fr(fin, notrunclabels, &rules);
+    if (fr.kind() == FastxReader::GZIP) { err = "gzip-compressed input is not supported"; }
+    else if (fr.kind() == FastxReader::BZIP2) { err = "bzip2-compressed input is not supported"; }
+    else { fr.fill(b, INT32_MAX, err); }
+  }
+  std::fclose(fin);
+  if (!err.empty()) { Error::set(std::string(caller) + ": " + err + " (" + path + ")"); return VSG_EINVAL; }
+  if (b.cat.empty()) { b.cat.push_back('\0'); }
+  out.cat = std::move(b.cat);
+  out.off = std::move(b.off);
+  out.len = std::move(b.len);
+  out.head = std::move(b.head);
+  out.stripped = rules.stripped;
+  out.discarded_short = rules.discarded_short;
+  out.discarded_long = rules.discarded_long;
+  return VSG_OK;
+}
+
 // The --makeudb_usearch command (commands/makeudb_usearch.cpp:105-273): the whole file parsed under db.read's rules, the
 // database made on the device (vsg_udb_make), the file written (vsg_udb_write).  The stages run one after another: the
 // file's word index, which comes before its sequences, needs every sequence.
@@ -595,23 +626,9 @@ extern "C" int vsg_makeudb_usearch(vsg_ctx * c, const char * input_path, const v
   if (rc != VSG_OK) { return rc; }
   auto const t_wall = std::chrono::steady_clock::now();
   vsg_makeudb_stats st{};
-  std::FILE * fin = std::fopen(input_path, "rb");
-  if (fin == nullptr) { Error::set(std::string("vsg_makeudb_usearch: cannot open ") + input_path); return VSG_EINVAL; }
-  FastxRules rules;
-  rules.symbols = true;
-  rules.minlen = std::max<int64_t>(opts->minseqlength, 0);
-  rules.maxlen = opts->maxseqlength;
-  StreamBatch b;
-  std::string err;
-  {
-    FastxReader fr(fin, opts->notrunclabels != 0, &rules);
-    if (fr.kind() == FastxReader::GZIP) { err = "gzip-compressed input is not supported"; }
-    else if (fr.kind() == FastxReader::BZIP2) { err = "bzip2-compressed input is not supported"; }
-    else { fr.fill(b, INT32_MAX, err); }
-  }
-  std::fclose(fin);
-  if (!err.empty()) { Error::set(std::string("vsg_makeudb_usearch: ") + err + " (" + input_path + ")"); return VSG_EINVAL; }
-  if (b.cat.empty()) { b.cat.push_back('\0'); }
+  FastxFile b;
+  rc = read_fastx_file("vsg_makeudb_usearch", input_path, opts->notrunclabels != 0, opts->minseqlength, opts->maxseqlength, b);
+  if (rc != VSG_OK) { return rc; }
   int64_t const n = static_cast<int64_t>(b.head.size());
   std::vector<const char *> heads(static_cast<size_t>(n));
   for (int64_t i = 0; i < n; i++) { heads[static_cast<size_t>(i)] = b.head[static_cast<size_t>(i)].c_str(); }
@@ -630,9 +647,9 @@ extern "C" int vsg_makeudb_usearch(vsg_ctx * c, const char * input_path, const v
   vsg_udb_close(u);
   if (rc != VSG_OK) { return rc; }
   st.sequences = n;
-  st.discarded_short = rules.discarded_short;
-  st.discarded_long = rules.discarded_long;
-  st.stripped = rules.stripped;
+  st.discarded_short = b.discarded_short;
+  st.discarded_long = b.discarded_long;
+  st.stripped = b.stripped;
   st.nucleotides = info.nucleotides;
   st.index_entries = info.index_entries;
   st.wall_s = seconds_since(t_wall);

@@ -202,6 +202,17 @@ int hits_out(const std::vector<vsg_search_result> & rows, const std::vector<int6
 // VSG_EINVAL (message prefixed with caller) for a word length outside 3..15 or an unknown dbmask (makeudb.cu)
 int makeudb_check_opts(const vsg_makeudb_opts * o, const char * caller);
 
+// every record of a FASTA or FASTQ file as db.read keeps it (stream.cu): the format from the first byte, gzip and bzip2
+// refused, core/fasta.cpp's symbol rules, labels cut at the first blank unless notrunclabels, records outside
+// [minlen, maxlen] discarded and counted (minlen < 1: no lower bound).  Errors are VSG_EINVAL, prefixed with caller.
+struct FastxFile {
+  std::vector<char> cat;             // sequences back to back, as read (case kept), then a NUL
+  std::vector<int64_t> off;
+  std::vector<int32_t> len;
+  std::vector<std::string> head;
+  int64_t stripped = 0, discarded_short = 0, discarded_long = 0;
+};
+int read_fastx_file(const char * caller, const char * path, bool notrunclabels, int64_t minlen, int64_t maxlen, FastxFile & out);
 // owning handle of a sequence set
 struct SeqsetDeleter { void operator()(vsg_seqset * s) const { vsg_seqset_destroy(s); } };
 using SeqsetPtr = std::unique_ptr<vsg_seqset, SeqsetDeleter>;

@@ -328,6 +328,17 @@ class Context:
                "vsg_makeudb_usearch")
         return {k: getattr(st, k) for k, _ in MakeudbStats._fields_}
 
+    def cluster_command(self, input_path: str, uc: Optional[str] = None, centroids: Optional[str] = None,
+                        clusters: Optional[str] = None, command: str = "cluster_fast", **opts) -> dict:
+        """vsg_cluster_command (--cluster_fast / _size / _smallmem / _unoise: a key of CLUSTER_COMMANDS): reads input_path,
+        writes --uc, --centroids and --clusters <prefix> (None: not written); opts as cluster_cmd_opts (id=0.97,
+        threads=8, qmask="soft", sizeout=1, ...).  Returns the stats as a dict."""
+        c, s = cluster_cmd_opts(command, **opts)
+        st = ClusterCmdStats()
+        _check(load().vsg_cluster_command(self.h, input_path.encode(), C.byref(c), C.byref(s),
+                                          *_cluster_cmd_paths(uc, centroids, clusters), C.byref(st)), "vsg_cluster_command")
+        return {k: getattr(st, k) for k, _ in ClusterCmdStats._fields_}
+
     def udb_load(self, udb: "Udb"):
         """vsg_udb_load: (SeqSetHandle, IndexHandle, mask_lower) of a parsed UDB file"""
         sh = C.c_void_p(); ih = C.c_void_p(); ml = C.c_int(-1)
@@ -440,6 +451,7 @@ def cluster_fast(ctx: "Context", ss: SeqSetHandle, opts: SearchOpts, round_size:
 _CLUSTER_DT = np.dtype([("cluster", np.int32), ("centroid", np.int32), ("matches", np.int32), ("mismatches", np.int32),
                         ("gaps", np.int32), ("alignment_length", np.int32), ("nwscore", np.int32), ("strand", np.int32),
                         ("id", np.float64)])
+CLUSTER_DT = _CLUSTER_DT   # one vsg_cluster_result
 
 
 class ClusterSession:
@@ -717,3 +729,74 @@ def makeudb_opts(**kw) -> MakeudbOpts:
             v = DBMASK[v]
         setattr(o, k, int(v))
     return o
+
+
+CLUSTER_COMMANDS = {"cluster_fast": 0, "cluster_size": 1, "cluster_smallmem": 2, "cluster_unoise": 3}
+
+
+class ClusterCmdOpts(C.Structure):
+    _fields_ = [("command", C.c_int32), ("threads", C.c_int32), ("qmask", C.c_int32), ("hardmask", C.c_int32),
+                ("usersort", C.c_int32), ("notrunclabels", C.c_int32), ("sizein", C.c_int32), ("sizeout", C.c_int32),
+                ("xsize", C.c_int32), ("clusterout_id", C.c_int32), ("clusterout_sort", C.c_int32), ("fasta_width", C.c_int32),
+                ("minseqlength", C.c_int64), ("maxseqlength", C.c_int64), ("minsize", C.c_int64), ("relabel", C.c_char_p)]
+
+
+class ClusterCmdStats(C.Structure):
+    _fields_ = [("sequences", C.c_int64), ("discarded_short", C.c_int64), ("discarded_long", C.c_int64),
+                ("discarded_minsize", C.c_int64), ("clusters", C.c_int64), ("singletons", C.c_int64), ("nucleotides", C.c_int64),
+                ("pairs", C.c_int64), ("cells", C.c_int64), ("parse_s", C.c_double), ("sort_s", C.c_double),
+                ("device_s", C.c_double), ("cigar_s", C.c_double), ("write_s", C.c_double), ("wall_s", C.c_double)]
+
+
+def cluster_cmd_opts(command: str = "cluster_fast", **kw):
+    """vsg_cluster_cmd_opts_default for `command` (a key of CLUSTER_COMMANDS), then the given fields: those of
+    vsg_cluster_cmd_opts go there (qmask may be "none" / "soft" / "dust", relabel a str), the rest to the search options.
+    Returns (ClusterCmdOpts, SearchOpts)."""
+    c, s = ClusterCmdOpts(), SearchOpts()
+    load().vsg_cluster_cmd_opts_default(C.c_int(CLUSTER_COMMANDS[command]), C.byref(c), C.byref(s))
+    names = {k for k, _ in ClusterCmdOpts._fields_}
+    for k, v in kw.items():
+        if k == "qmask" and isinstance(v, str):
+            v = DBMASK[v]
+        if k == "relabel":
+            c.relabel = v.encode() if isinstance(v, str) else v
+        elif k in names:
+            setattr(c, k, int(v))
+        else:
+            setattr(s, k, v)
+    return c, s
+
+
+def _cluster_cmd_paths(uc, centroids, clusters):
+    return tuple(p.encode() if p is not None else None for p in (uc, centroids, clusters))
+
+
+def cluster_write(headers, seqs, abundances, results: np.ndarray, cigars, uc: Optional[str] = None,
+                  centroids: Optional[str] = None, clusters: Optional[str] = None, command: str = "cluster_fast", **opts) -> int:
+    """vsg_cluster_write (host only, no device): the output files of records in processing order; `seqs` as printed
+    (bytes each), `results` a cluster result array (cluster_fast's dtype), `cigars` the CIGAR (str) of each H record
+    (anything for S records).  opts as cluster_cmd_opts.  Returns the number of singleton clusters."""
+    c, _ = cluster_cmd_opts(command, **opts)
+    n = len(headers)
+    res = np.ascontiguousarray(results, dtype=_CLUSTER_DT)
+    cat = np.frombuffer(b"".join(seqs) + b"\0", dtype=np.uint8)
+    ln = np.array([len(x) for x in seqs], dtype=np.int32)
+    off = np.zeros(n, dtype=np.int64)
+    if n > 1:
+        off[1:] = np.cumsum(ln[:-1], dtype=np.int64)
+    cig = [(x or "").encode() + b"\0" for x in cigars]
+    cbuf = np.frombuffer(b"".join(cig) + b"\0", dtype=np.uint8)
+    coff = np.zeros(max(n, 1), dtype=np.int64)
+    if n > 1:
+        coff[1:n] = np.cumsum([len(x) for x in cig[:-1]], dtype=np.int64)
+    ab = np.ascontiguousarray(abundances, dtype=np.int64)
+    single = C.c_int64()
+    _check(load().vsg_cluster_write(C.c_int64(n), _strings(headers) if n else None, cat.ctypes.data_as(C.c_char_p),
+                                    _ptr(off, C.c_int64), _ptr(ln, C.c_int32), _ptr(ab, C.c_int64),
+                                    res.ctypes.data_as(C.POINTER(ClusterResult)), cbuf.ctypes.data_as(C.c_char_p),
+                                    _ptr(coff, C.c_int64), C.byref(c), *_cluster_cmd_paths(uc, centroids, clusters),
+                                    C.byref(single)), "vsg_cluster_write")
+    return int(single.value)
+
+
+
