@@ -8,6 +8,8 @@
  *                (src/core/unique.cpp:155-353, dbindex.cpp:121-255,
  *                 searchcore.cpp:260-464, 541-957, minheap.cpp:82-263)
  *   - nt_maps.c: nucleotide code tables (src/utils/maps.cpp:75-118, 153-266)
+ *   - sintax.c : SINTAX's bootstraps for one query (src/commands/sintax.cpp:299-507),
+ *                pinned in tests/test_sintax_oracle_cpu.py
  *
  * Parity status: PINNED.  tests/test_oracle_vs_ref.py checks every function here
  * against the unmodified reference compiled into oracle/_ref/libvsref.so
@@ -76,6 +78,10 @@ oracle_index * oracle_index_build(int k, int n, const char * cat, const int64_t 
 void oracle_index_starts(const oracle_index * ix, uint64_t * start);
 void oracle_index_postings(const oracle_index * ix, uint32_t * post);
 void oracle_index_free(oracle_index * ix);
+int oracle_index_wordlength(const oracle_index * ix);
+int oracle_index_count(const oracle_index * ix);   /* indexed targets */
+/* the postings of k-mer km: *n ascending target numbers */
+const uint32_t * oracle_index_list(const oracle_index * ix, uint32_t km, uint64_t * n);
 
 /* search_topscores: best-first (count desc, length asc, seqno asc) list of at most
    tophits targets with count >= min(minwordmatches, nkmers).  Returns the count. */
@@ -117,6 +123,30 @@ int oracle_search_onequery(const oracle_index * ix, const oracle_scoring * sc,
                            const char * q, int qlen, int strand,
                            oracle_hit * hits_out, int hits_cap,
                            int64_t * pairs_aligned, int64_t * cells_aligned);
+
+/* sintax.c — the bootstraps of one query (sintax_query + sintax_search_topscores, src/commands/sintax.cpp:299-507)
+   against the index of the whole database.  out is laid out as vsg_sintax_result: out[0] = strand, out[1..2] =
+   successful bootstraps per strand, out[3..4] = largest winning count per strand, out[5 + 100 * s + i] = winner i of
+   strand s (-1 beyond the successful ones). */
+#define ORACLE_SINTAX_BOOTSTRAPS 100
+#define ORACLE_SINTAX_SUBSET 32
+void oracle_sintax(const oracle_index * ix, const int * target_len, const char * q, int qlen,
+                   uint64_t query_number, uint64_t seed, int strand_both, int32_t out[205]);
+
+/* one bootstrap as oracle_sintax saw it */
+typedef struct oracle_sintax_boot {
+  int32_t winner;            /* -1: no draws, or no target holds two of the sampled k-mers */
+  int32_t count;             /* the largest count of any target */
+  int32_t ntied;             /* targets with that count */
+  int32_t tied_lo, tied_hi;  /* the lowest and the highest number among them */
+  int32_t nsamp;             /* distinct sampled k-mers */
+  uint32_t samp[ORACLE_SINTAX_SUBSET];
+} oracle_sintax_boot;
+
+/* oracle_sintax, and (trace != NULL) every bootstrap of strand s at trace[100 * s + b] */
+void oracle_sintax_trace(const oracle_index * ix, const int * target_len, const char * q, int qlen,
+                         uint64_t query_number, uint64_t seed, int strand_both, int32_t out[205],
+                         oracle_sintax_boot * trace);
 
 #ifdef __cplusplus
 }

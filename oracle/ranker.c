@@ -176,6 +176,18 @@ void oracle_index_free(oracle_index * ix)
   if (ix) { free(ix->start); free(ix->keys); free(ix->post); free(ix); }
 }
 
+int oracle_index_wordlength(const oracle_index * ix) { return ix->k; }
+
+int oracle_index_count(const oracle_index * ix) { return ix->n; }
+
+const uint32_t * oracle_index_list(const oracle_index * ix, uint32_t km, uint64_t * n)
+{
+  uint64_t a, b;
+  oracle_list(ix, km, &a, &b);
+  *n = b - a;
+  return ix->post + a;
+}
+
 typedef struct { uint32_t count, seqno, length; } elem;
 
 /* best first: count desc, length asc, seqno asc (minheap_compare reversed, minheap.cpp:108-136) */

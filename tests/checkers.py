@@ -253,6 +253,7 @@ class OracleDb:
     def __init__(self, ss, k=8, mask_lower=0):
         self.ss = ss
         self.k = k
+        self.mask_lower = mask_lower
         self.h = oracle().oracle_index_build(C.c_int(k), C.c_int(len(ss)), _p(ss.cat, C.c_char),
                                              _p(ss.offs, C.c_int64), _p(ss.lens, C.c_int),
                                              C.c_int(mask_lower))
@@ -283,6 +284,21 @@ class OracleDb:
                                             hits, C.c_int(opts.tophits + 1),
                                             C.byref(pairs), C.byref(cells))
         return [hits[i] for i in range(n)], pairs.value, cells.value
+
+    def sintax(self, q: bytes, query_number: int, seed: int, strand_both: int = 0, trace: bool = False):
+        """oracle_sintax: the bootstraps of one query as a 205-int row laid out as vsg_sintax_result; with trace, also
+        every bootstrap (SintaxBoot * 200, strand s at [100 * s + b])"""
+        out = np.zeros(205, dtype=np.int32)
+        tr = (SintaxBoot * 200)() if trace else None
+        oracle().oracle_sintax_trace(C.c_void_p(self.h), _p(self.ss.lens, C.c_int), q, C.c_int(len(q)),
+                                     C.c_uint64(query_number), C.c_uint64(seed), C.c_int(strand_both),
+                                     _p(out, C.c_int32), tr)
+        return (out, tr) if trace else out
+
+
+class SintaxBoot(C.Structure):
+    _fields_ = [("winner", C.c_int32), ("count", C.c_int32), ("ntied", C.c_int32), ("tied_lo", C.c_int32),
+                ("tied_hi", C.c_int32), ("nsamp", C.c_int32), ("samp", C.c_uint32 * 32)]
 
 
 class RefDb:

@@ -147,6 +147,72 @@ def ref_bootstraps(case):
     return out
 
 
+SHARD = 32766   # targets per static index shard
+
+
+def _repeat_tail(s: bytes) -> bytes:
+    """s with its last 20 nt repeated: at every k <= 20 it holds the same k-mers as itself one base shorter"""
+    return s + s[-20:]
+
+
+@functools.lru_cache(maxsize=None)
+def three_shard_data(n: int = 70_001, seed: int = 4242):
+    """A database of `n` targets, so three static index shards, the last one partial with an odd number of targets:
+    random background sequences of 100-260 nt, and 20 families of 2-6 % variants of 400-nt roots spread over the whole
+    database.  Planted across the shards (each pair holds the same k-mers at every k, so only length and number can
+    decide between them):
+      - an exact copy in shard 2 of a member in shard 1 (the shard-1 one wins: same length, lower number);
+      - in shard 2, a copy one base shorter of a member in shard 0 (the shard-2 one wins: shorter);
+      - one base shorter / longer pairs on either side of both shard boundaries, and the last target (the low half of
+        the last counter word of the partial shard) one base shorter than a target in shard 0.
+    Queries: 2 % variants of 200-nt windows of the planted members (one of each pair reverse-complemented), of members
+    of the other families, random sequences and one too short for bootstraps.
+    Returns dict(db_seqs, q_seqs, meta) with meta["never"]: targets that can never win a bootstrap, meta["wins"]:
+    their partners."""
+    rng = np.random.default_rng(seed)
+    lens = rng.integers(100, 261, size=n)
+    m = synth.random_seqs(rng, n, 260)
+    seqs = [m[i, :lens[i]].tobytes() for i in range(n)]
+    roots = synth.random_seqs(rng, 20, 400)
+    fam = {}
+    for f in range(20):
+        idx = rng.choice(n, size=30, replace=False)
+        fam[f] = idx
+        for i in idx:
+            seqs[i] = synth.mutate(rng, roots[f], float(rng.uniform(0.02, 0.06))).tobytes()
+    last = n - 1
+    planted = {}   # family: (winner, loser, sequence of the winner, sequence of the loser)
+
+    def member(f):
+        return _repeat_tail(synth.mutate(rng, roots[f], 0.02).tobytes())
+
+    x = synth.mutate(rng, roots[1], 0.02).tobytes()
+    planted[1] = (40_000, 68_000, x, x)                          # exact copies in shards 1 and 2
+    y = member(2)
+    planted[2] = (69_000, 5_000, y[:-1], y)                      # shorter copy in shard 2 of a shard-0 member
+    w = member(3)
+    planted[3] = (SHARD, SHARD - 1, w[:-1], w)                   # across the 0 | 1 boundary: the higher number is shorter
+    v = member(4)
+    planted[4] = (2 * SHARD - 1, 2 * SHARD, v[:-1], v)           # across the 1 | 2 boundary: the lower number is shorter
+    u = member(5)
+    planted[5] = (last, 100, u[:-1], u)                          # the last target against a shard-0 one
+    for f, (win, lose, sw, sl) in planted.items():
+        seqs[win], seqs[lose] = sw, sl
+    queries = []
+    for f, (win, lose, sw, _) in planted.items():
+        for j in range(2):
+            p = int(rng.integers(0, len(sw) - 240))
+            qv = synth.mutate(rng, np.frombuffer(sw[p:p + 200], dtype=np.uint8), 0.02).tobytes()
+            queries.append(synth.revcomp(qv) if j else qv)
+    for f in range(6, 20):
+        s = seqs[int(fam[f][int(rng.integers(0, 30))])]
+        p = int(rng.integers(0, len(s) - 200))
+        queries.append(synth.mutate(rng, np.frombuffer(s[p:p + 200], dtype=np.uint8), 0.02).tobytes())
+    queries += [r.tobytes() for r in synth.random_seqs(rng, 3, 200)] + [b"ACGTTGCAACGTAGGC"]
+    meta = {"never": [p[1] for p in planted.values()], "wins": [p[0] for p in planted.values()]}
+    return {"db_seqs": seqs, "q_seqs": queries, "meta": meta}
+
+
 def as_array(res):
     """Context.sintax's dict -> the (nq, 205) layout of ref_bootstraps"""
     n = res["strand"].shape[0]
