@@ -363,6 +363,23 @@ int vsg_cluster_session_assign(vsg_cluster_session * session, int64_t start, int
 int64_t vsg_cluster_session_clusters(const vsg_cluster_session * session);
 void vsg_cluster_session_destroy(vsg_cluster_session * session);
 
+/* ---- the cluster driver's own index of the centroids, exposed for tests: the incremental k-mer index that
+ *      vsg_cluster_fast, cluster sessions and vsg_cluster_command grow as centroids are created (shards of 32 768
+ *      targets; wordlength 3..10).  Every list capacity is sized from the whole `set`, which must outlive the index.
+ *      vsg_cluster_index_append adds the sequences seqnos[0 .. n) as new targets; their numbers must be strictly
+ *      ascending, after the last one appended and inside the set (VSG_EINVAL otherwise).  Targets get DENSE numbers in
+ *      append order, and vsg_cluster_index_rank returns those: as vsg_rank, for every query of `queries` in [q0, q0+nq)
+ *      the best-first list (count desc, target length asc, dense number asc) of at most tophits targets with count >=
+ *      min(minwordmatches, distinct query k-mers), with the index's mask_lower on the query side; tophits > 1024 takes
+ *      the unbounded lists. ---- */
+typedef struct vsg_cluster_index vsg_cluster_index;
+int vsg_cluster_index_create(vsg_ctx * ctx, const vsg_seqset * set, int wordlength, int mask_lower, vsg_cluster_index ** out);
+int vsg_cluster_index_append(vsg_ctx * ctx, vsg_cluster_index * ix, const uint32_t * seqnos, int64_t n);
+int64_t vsg_cluster_index_count(const vsg_cluster_index * ix);
+int vsg_cluster_index_rank(vsg_ctx * ctx, vsg_cluster_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
+                           int minwordmatches, int tophits, uint32_t * cand, uint32_t * count, int32_t * ncand);
+void vsg_cluster_index_destroy(vsg_cluster_index * ix);
+
 /* ---- several GPUs behind one process (SURVEY.md §8e; the reference is a single process, LIBRARY_API.md:138-156):
  *      vsg_group_create uploads the database ONCE (to devices[0]; dust_db != 0 also DUST-masks it there,
  *      core/mask.cpp dust_all), copies the packed sequences device to device over NVLink to every other GPU and

@@ -1296,3 +1296,95 @@ int cindex_rank_lists(vsg_ctx * c, CIndex * ix, const vsg_seqset * queries, int6
 }
 
 }  // namespace vsg
+
+// ---- the cluster driver's incremental index on its own (include/vsg.h), so its candidate lists can be compared with a
+//      plain index of the same targets ----
+struct vsg_cluster_index {
+  vsg::CIndex * ix = nullptr;
+  int64_t nseq = 0;        // sequences in the set
+  int64_t last = -1;       // the last sequence number appended
+};
+
+extern "C" int vsg_cluster_index_create(vsg_ctx * c, const vsg_seqset * set, int wordlength, int mask_lower, vsg_cluster_index ** out)
+{
+  if (c == nullptr || set == nullptr || out == nullptr) { Error::set("vsg_cluster_index_create: null argument"); return VSG_EINVAL; }
+  *out = nullptr;
+  if (set->device != c->device) { Error::set("vsg_cluster_index_create: sequence set lives on another device than the context"); return VSG_EINVAL; }
+  vsg_cluster_index * h = new (std::nothrow) vsg_cluster_index();
+  if (h == nullptr) { Error::set("out of host memory"); return VSG_ENOMEM; }
+  int const rc = cindex_create(c, set, wordlength, mask_lower, &h->ix);
+  if (rc != VSG_OK) { delete h; return rc; }
+  h->nseq = set->d.n;
+  *out = h;
+  return VSG_OK;
+}
+
+extern "C" int vsg_cluster_index_append(vsg_ctx * c, vsg_cluster_index * h, const uint32_t * seqnos, int64_t n)
+{
+  if (c == nullptr || h == nullptr || (n > 0 && seqnos == nullptr)) { Error::set("vsg_cluster_index_append: null argument"); return VSG_EINVAL; }
+  if (n < 0 || n > INT32_MAX) { Error::set("vsg_cluster_index_append: count out of range"); return VSG_EINVAL; }
+  if (h->ix->device != c->device) { Error::set("vsg_cluster_index_append: index lives on another device than the context"); return VSG_EINVAL; }
+  // cindex_append takes new targets in ascending sequence order, each once, after every earlier one
+  int64_t prev = h->last;
+  for (int64_t i = 0; i < n; i++) {
+    int64_t const s = seqnos[i];
+    if (s <= prev || s >= h->nseq) {
+      Error::set("vsg_cluster_index_append: sequence numbers must be strictly ascending, after the last one appended and inside the set");
+      return VSG_EINVAL;
+    }
+    prev = s;
+  }
+  VSG_CUDA_OK(cudaSetDevice(c->device));
+  int const rc = cindex_append(c, h->ix, seqnos, static_cast<int>(n));
+  if (rc != VSG_OK) { return rc; }
+  VSG_CUDA_OK(cudaGetLastError());
+  h->last = prev;
+  return VSG_OK;
+}
+
+extern "C" int64_t vsg_cluster_index_count(const vsg_cluster_index * h)
+{
+  return h == nullptr ? 0 : static_cast<int64_t>(cindex_seqnos(h->ix).size());
+}
+
+extern "C" int vsg_cluster_index_rank(vsg_ctx * c, vsg_cluster_index * h, const vsg_seqset * queries, int64_t q0, int64_t nq,
+                                      int minwordmatches, int tophits, uint32_t * cand, uint32_t * count, int32_t * ncand)
+{
+  if (c == nullptr || h == nullptr || queries == nullptr || (nq > 0 && (cand == nullptr || count == nullptr || ncand == nullptr))) {
+    Error::set("vsg_cluster_index_rank: null argument");
+    return VSG_EINVAL;
+  }
+  if (tophits < 1) { Error::set("vsg_cluster_index_rank: tophits must be at least 1"); return VSG_EINVAL; }
+  if (q0 < 0 || nq < 0 || q0 + nq > queries->d.n) { Error::set("vsg_cluster_index_rank: query range out of bounds"); return VSG_EINVAL; }
+  if (queries->device != c->device || h->ix->device != c->device) {
+    Error::set("vsg_cluster_index_rank: sequence set / index lives on another device than the context");
+    return VSG_EINVAL;
+  }
+  if (nq > (1 << 30) / tophits) { Error::set("vsg_cluster_index_rank: batch too large"); return VSG_EINVAL; }
+  VSG_CUDA_OK(cudaSetDevice(c->device));
+  int rc;
+  if (tophits > TOPHITS_MAX) {
+    std::vector<int64_t> first;
+    std::vector<uint32_t> seqno, cnt;
+    if ((rc = cindex_rank_lists(c, h->ix, queries, q0, nq, minwordmatches, tophits, first, seqno, cnt)) != VSG_OK) { return rc; }
+    for (int64_t i = 0; i < nq; i++) {
+      size_t const a = static_cast<size_t>(first[static_cast<size_t>(i)]), n = static_cast<size_t>(first[static_cast<size_t>(i) + 1]) - a;
+      std::memcpy(cand + static_cast<size_t>(i) * tophits, seqno.data() + a, sizeof(uint32_t) * n);
+      std::memcpy(count + static_cast<size_t>(i) * tophits, cnt.data() + a, sizeof(uint32_t) * n);
+      ncand[i] = static_cast<int32_t>(n);
+    }
+    return VSG_OK;
+  }
+  RankTop r;
+  if ((rc = cindex_rank_enqueue(c, h->ix, queries, q0, nq, minwordmatches, tophits, r)) != VSG_OK ||
+      (rc = rank_download(c, r, nq, tophits, cand, count, ncand, "vsg_cluster_index_rank")) != VSG_OK) { return rc; }
+  VSG_CUDA_OK(cudaGetLastError());
+  return VSG_OK;
+}
+
+extern "C" void vsg_cluster_index_destroy(vsg_cluster_index * h)
+{
+  if (h == nullptr) { return; }
+  cindex_destroy(h->ix);
+  delete h;
+}

@@ -247,14 +247,16 @@ __device__ __forceinline__ void postings_stream(const ShardDev & S, int n, uint3
 //    range visit each thread's counters in the same order.  W = 4 (one 16-byte load) for the scans of the running
 //    threshold and the unbounded ranker; W = 1 for the fixed-threshold scans, whose appends keep more state live
 //    (four words per thread there spill).  zero: the words are cleared behind the scan, and so is the word the padding
-//    entries of the lists land in (the next shard then skips its clearing pass).
+//    entries of the lists land in (the next shard then skips its clearing pass).  That word holds the counters of
+//    targets 32766 and 32767 in an incremental shard of more than SHARD_STATIC targets: there the scan itself reads and
+//    clears it, and clearing it up front would race with that read.
 template <int W, typename F>
 __device__ __forceinline__ void visit_counters(uint32_t * counters, int w0, int w1, int nt, uint32_t thr, bool zero, F && f)
 {
   static_assert(W == 1 || W == 4, "counter words per load");
   int const v1 = (w1 + W - 1) / W;
   uint32_t const below = thr > 0 ? ((thr - 1) | ((thr - 1) << 16)) : 0u;
-  if (zero && threadIdx.x == 0) { counters[(POST_PAD >> 2)] = 0; }
+  if (zero && threadIdx.x == 0 && nt <= SHARD_STATIC) { counters[(POST_PAD >> 2)] = 0; }
   for (int vi = w0 / W + threadIdx.x; vi < v1; vi += blockDim.x) {
     uint32_t w[W];
     if constexpr (W == 4) {

@@ -162,6 +162,44 @@ class IndexHandle:
             self.h = None
 
 
+class ClusterIndex:
+    """vsg_cluster_index: the cluster driver's incremental index, grown by append(seqnos); rank() returns DENSE target
+    numbers (append order)"""
+
+    def __init__(self, ctx: "Context", ss: SeqSetHandle, wordlength: int, mask_lower: int):
+        self._keep = (ctx, ss)
+        self.ctx = ctx
+        self.h = C.c_void_p()
+        lib = load()
+        lib.vsg_cluster_index_count.restype = C.c_int64
+        _check(lib.vsg_cluster_index_create(ctx.h, ss.h, C.c_int(wordlength), C.c_int(mask_lower), C.byref(self.h)),
+               "vsg_cluster_index_create")
+
+    def append(self, seqnos):
+        s = np.ascontiguousarray(seqnos, dtype=np.uint32)
+        _check(load().vsg_cluster_index_append(self.ctx.h, self.h, _ptr(s, C.c_uint32), C.c_int64(s.shape[0])),
+               "vsg_cluster_index_append")
+
+    @property
+    def count(self) -> int:
+        return int(load().vsg_cluster_index_count(self.h))
+
+    def rank(self, qs: SeqSetHandle, q0: int, nq: int, minwordmatches: int, tophits: int):
+        """(cand[nq, tophits], count[nq, tophits], ncand[nq]) as Context.rank, candidates as dense numbers"""
+        cand = np.zeros((nq, tophits), dtype=np.uint32)
+        count = np.zeros((nq, tophits), dtype=np.uint32)
+        nc = np.zeros(nq, dtype=np.int32)
+        _check(load().vsg_cluster_index_rank(self.ctx.h, self.h, qs.h, C.c_int64(q0), C.c_int64(nq), C.c_int(minwordmatches),
+                                             C.c_int(tophits), _ptr(cand, C.c_uint32), _ptr(count, C.c_uint32),
+                                             _ptr(nc, C.c_int32)), "vsg_cluster_index_rank")
+        return cand, count, nc
+
+    def close(self):
+        if self.h:
+            load().vsg_cluster_index_destroy(self.h)
+            self.h = C.c_void_p()
+
+
 class Context:
     """vsg_ctx: one CUDA stream + scratch; mirrors the reference's per-thread s16info_s."""
 
@@ -304,6 +342,10 @@ class Context:
         _check(load().vsg_index_create(self.h, db.h, C.c_int(wordlength), C.c_int(mask_lower),
                                        C.byref(h)), "vsg_index_create")
         return IndexHandle(h)
+
+    def cluster_index(self, ss: SeqSetHandle, wordlength: int = 8, mask_lower: int = 0) -> "ClusterIndex":
+        """vsg_cluster_index_create: the cluster driver's incremental index over sequences of `ss`, empty at first"""
+        return ClusterIndex(self, ss, wordlength, mask_lower)
 
     def udb_make(self, seqs, headers, wordlength=8, dbmask="dust", hardmask=False) -> "Udb":
         """vsg_udb_make: the in-memory UDB database of the records `seqs` (bytes each) with `headers` (str each)"""
