@@ -631,6 +631,80 @@ int vsg_cluster_write(int64_t n, const char * const * headers, const char * cat,
                       const int64_t * cigar_off, const vsg_cluster_cmd_opts * c, const char * uc, const char * centroids,
                       const char * clusters_prefix, int64_t * singletons);
 
+/* ---- exact-match search: replaces Dbhash (core/dbhash.cpp) and search_exact_onequery / add_hit
+ *      (commands/search_exact.cpp:136-209).  vsg_exact_index_create hashes every sequence of `db` on the device (the
+ *      4-bit codes and the length, so case and U / T do not matter and N only equals N, as seqcmp compares) and keeps the
+ *      (hash, sequence number) pairs sorted: 12 bytes per target.  `db` must outlive the index.  vsg_search_exact finds, for
+ *      every query of `queries` in [q0, q0 + nq) and with strand_both also for its reverse complement, every database
+ *      sequence identical to it: the candidates of equal hash are all compared symbol by symbol.  Each match becomes the
+ *      hit add_hit makes (100 % identity, nwscore = query length * match score, no gaps, no trims) and passes the two
+ *      accept functions with --id 1.0; the size / length / idprefix / idsuffix / self / selfid filters, query_sizes /
+ *      target_sizes and query_labels / target_labels of opts apply as for vsg_search_hits.  opts->id, maxaccepts,
+ *      maxrejects, wordlength and iddef are ignored: every identical target is reported.  The rows of query q0 + i are
+ *      hits[first[i] .. first[i+1]) (first: nq + 1 offsets), at most maxhits of them (0: all), in search_joinhits order
+ *      (target ascending; a palindrome's two hits on one target plus strand first).  *nhits receives the number of rows;
+ *      above cap the call returns VSG_ECAP with first filled and hits untouched.
+ *      VSG_EXACT_HASH_BITS (environment, read at index creation; unset = 64) keeps only the low bits of every hash, which
+ *      forces collisions through the comparison (a test aid; results are the same). ---- */
+typedef struct vsg_exact_index vsg_exact_index;
+int vsg_exact_index_create(vsg_ctx * ctx, const vsg_seqset * db, vsg_exact_index ** out);
+void vsg_exact_index_destroy(vsg_exact_index * ix);
+int vsg_search_exact(vsg_ctx * ctx, const vsg_exact_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
+                     const vsg_search_opts * opts, int64_t maxhits, vsg_search_result * hits, int64_t cap, int64_t * first,
+                     int64_t * nhits);
+
+/* ---- the --search_exact command: replaces search_exact() (commands/search_exact.cpp:211-908).  The database is read
+ *      whole as db.read keeps it (FASTA or FASTQ, gzip / bzip2 and UDB files refused, labels cut at the first blank unless
+ *      notrunclabels, records outside [minseqlength, maxseqlength] discarded and counted); with dbmask soft + hardmask
+ *      its lower case becomes 'N'.  Queries (FASTA or FASTQ) stream in batches of batch_queries over a reader thread, the
+ *      device (upload, soft + hardmask as 'N' on the host, vsg_search_exact with query_sizes from ";size=", --self label
+ *      identities) and a writer thread that writes the rows in input order (the reference's order with --threads 1):
+ *      --blast6out (at most maxhits rows per query, the "*" row with output_no_hits), --uc (H rows: the first hit, or
+ *      every reported hit with uc_allhits; an N row for a query without a hit), --matched / --notmatched (the query as
+ *      masked: with qmask dust, DUST on the device, masked symbols lower case and the rest upper case).  At the end:
+ *      --dbmatched / --dbnotmatched (the database as masked by dbmask, DUST on the device; with sizeout the abundance is
+ *      the query abundance summed over the accepted hits with sizein, the number of accepted hits without), and the OTU
+ *      tables --otutabout / --mothur_shared_out (core/otutable.cpp: the query's sample from "sample=" / "barcodelabel=",
+ *      else its leading [A-Za-z0-9_] run; the OTU from the first hit's "otu=", else its label up to the first ';'; "tax="
+ *      gives the taxonomy column; the query abundance from ";size=" counts; unmatched targets are added with 0).
+ *      DUST runs only when a file printing masked sequences asks for it; matching never depends on case.  Any output path
+ *      may be NULL; a failed call leaves none of the files it made.  Refused with VSG_EINVAL and no file: no output, gzip
+ *      or bzip2 input, a UDB database, qmask or dbmask dust with hardmask (the device DUST would upper-case the rest first),
+ *      a missing file.  Not offered: --alnout, --samout, --userout, --fastapairs, --qsegout, --tsegout, --biomout, --lcaout,
+ *      --relabel*, --label_suffix, --sample, --lengthout, --xee, several GPUs.  s carries strand_both and the filters of
+ *      vsg_search_exact; its size and label arrays are the command's own (pass them NULL).
+ *      vsg_search_exact_opts_default fills the CLI's defaults for --search_exact (cli.cc): dbmask and qmask dust,
+ *      minseqlength 1, maxseqlength 50 000, fasta_width 80, maxhits 0 (all), batch_queries 65 536. ---- */
+typedef struct vsg_search_exact_opts {
+  int32_t dbmask;           /* --dbmask: VSG_DBMASK_NONE / _SOFT / _DUST (default dust) */
+  int32_t qmask;            /* --qmask (default dust) */
+  int32_t hardmask;         /* --hardmask (with soft: lower case becomes 'N'; refused with dust) */
+  int32_t sizein;           /* --sizein: --dbmatched abundances sum the query abundances */
+  int32_t sizeout;          /* --sizeout */
+  int32_t xsize;            /* --xsize */
+  int32_t notrunclabels;    /* --notrunclabels */
+  int32_t fasta_width;      /* --fasta_width (default 80; 0: one line) */
+  int64_t minseqlength;     /* --minseqlength (default 1) */
+  int64_t maxseqlength;     /* --maxseqlength (default 50 000) */
+  int64_t maxhits;          /* --maxhits (0: all) */
+  int32_t uc_allhits;       /* --uc_allhits */
+  int32_t output_no_hits;   /* --output_no_hits */
+  int32_t batch_queries;    /* queries per device call (default 65 536) */
+  int32_t reserved;
+} vsg_search_exact_opts;
+typedef struct vsg_search_exact_outputs {
+  const char * blast6out, * uc, * matched, * notmatched, * dbmatched, * dbnotmatched, * otutabout, * mothur_shared_out;
+} vsg_search_exact_outputs;
+typedef struct vsg_search_exact_stats {
+  int64_t queries, matched;                     /* "Matching unique query sequences: matched of queries" */
+  int64_t queries_abundance, matched_abundance; /* "Matching total query sequences" (printed with --sizein) */
+  int64_t db_sequences, db_discarded_short, db_discarded_long, hits;
+  double parse_s, device_s, write_s, wall_s;
+} vsg_search_exact_stats;
+void vsg_search_exact_opts_default(vsg_search_exact_opts * e, vsg_search_opts * s);
+int vsg_search_exact_command(vsg_ctx * ctx, const char * query_path, const char * db_path, const vsg_search_exact_opts * e,
+                             const vsg_search_opts * s, const vsg_search_exact_outputs * outputs, vsg_search_exact_stats * stats);
+
 #ifdef __cplusplus
 }
 #endif

@@ -3,6 +3,7 @@
 
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <cstdio>
 #include <memory>
 #include <string>
 #include <vector>
@@ -213,6 +214,46 @@ struct FastxFile {
   int64_t stripped = 0, discarded_short = 0, discarded_long = 0;
 };
 int read_fastx_file(const char * caller, const char * path, bool notrunclabels, int64_t minlen, int64_t maxlen, FastxFile & out);
+// The reference's label and FASTA writers as the commands use them (cluster_cmd.cu).
+// header_find_attribute: the first "(^|;)size=[0-9]+(;|$)" of the label; [start, end) covers "size=<digits>"
+bool find_size(const std::string & h, int & start, int & end);
+// fastx_get_abundance / header_get_size: 1 without an annotation; zero or out of range is an error (false, err set)
+bool abundance_of(const std::string & h, int64_t & out, std::string & err);
+// header_fprint_strip with only --xsize among the stripped attributes; returns whether the last character written is ';'
+bool header_fprint_strip(std::string & out, const std::string & h, bool strip_size);
+// fasta_print_general with the options the commands offer: --relabel prefix (used when ordinal > 0, NULL: none),
+// --xsize, --sizeout (";size=" when abundance > 0), ";clusterid=" (clusterid >= 0), fasta_width (< 1: one line)
+struct FastaFormat {
+  const char * relabel;
+  bool xsize, sizeout;
+  int fasta_width;
+};
+void fasta_print_general(std::string & out, const FastaFormat & f, const std::string & head, const char * seq, int64_t len,
+                         int64_t abundance, int64_t ordinal, int64_t clusterid);
+// the files a call creates, removed again unless the call succeeds
+struct OutFiles {
+  std::vector<std::string> made;
+  bool ok = false;
+  ~OutFiles() { if (!ok) { for (auto const & p : made) { std::remove(p.c_str()); } } }
+  bool write(const std::string & path, const std::string & data)
+  {
+    std::FILE * f = std::fopen(path.c_str(), "wb");
+    if (f == nullptr) { return false; }
+    made.push_back(path);
+    bool const good = std::fwrite(data.data(), 1, data.size(), f) == data.size();
+    return std::fclose(f) == 0 && good;
+  }
+};
+// results_show_blast6out_one (core/results.cpp:221-271): the --blast6out rows of one query's n hits, or with n == 0 and
+// output_no_hits its "*" row; returns the rows written (stream.cu)
+int64_t blast6_rows(std::string & out, const std::string & qhead, const vsg_search_result * r, int64_t n,
+                    const char * const * target_labels, bool output_no_hits);
+
+// vsg_search_exact with the rows kept on the host: query i's are rows[first[i] .. first[i + 1]) (exact.cu)
+int search_exact_host(vsg_ctx * c, const vsg_exact_index * ix, const vsg_seqset * queries, int64_t q0, int64_t nq,
+                      const vsg_search_opts * opts, int64_t maxhits, std::vector<vsg_search_result> & rows,
+                      std::vector<int64_t> & first);
+
 // owning handle of a sequence set
 struct SeqsetDeleter { void operator()(vsg_seqset * s) const { vsg_seqset_destroy(s); } };
 using SeqsetPtr = std::unique_ptr<vsg_seqset, SeqsetDeleter>;

@@ -381,6 +381,31 @@ class Context:
                                           *_cluster_cmd_paths(uc, centroids, clusters), C.byref(st)), "vsg_cluster_command")
         return {k: getattr(st, k) for k, _ in ClusterCmdStats._fields_}
 
+    def exact_index(self, db: SeqSetHandle) -> "ExactIndex":
+        """vsg_exact_index_create: the hash index of every sequence of `db` (which must outlive it)"""
+        h = C.c_void_p()
+        _check(load().vsg_exact_index_create(self.h, db.h, C.byref(h)), "vsg_exact_index_create")
+        return ExactIndex(h)
+
+    def search_exact(self, ix: "ExactIndex", qs: SeqSetHandle, q0: int, nq: int, opts: SearchOpts, maxhits: int = 0,
+                     cap: Optional[int] = None):
+        """vsg_search_exact -> (rows, first[nq + 1], work[4], unused); query i's rows are rows[first[i]:first[i + 1]].
+        cap=None: the buffer is sized by a first call that reports the number of rows (VSG_ECAP)."""
+        return _hits_call(lambda hits, c, first, n, _work: load().vsg_search_exact(
+            self.h, ix.h, qs.h, C.c_int64(q0), C.c_int64(nq), C.byref(opts), C.c_int64(maxhits), hits, C.c_int64(c), first, n),
+            nq, cap, "vsg_search_exact")
+
+    def search_exact_command(self, query_path: str, db_path: str, /, **kw) -> dict:
+        """vsg_search_exact_command (--search_exact): keywords naming an output of SearchExactOutputs give its path, those
+        of vsg_search_exact_opts its value (qmask / dbmask may be "none" / "soft" / "dust"), the rest go to the search
+        options (strand_both, self, mintsize, ...; the arguments before them are positional-only, so `self` can be one).
+        Returns the stats as a dict."""
+        e, s, o = search_exact_opts(**kw)
+        st = SearchExactStats()
+        _check(load().vsg_search_exact_command(self.h, query_path.encode(), db_path.encode(), C.byref(e), C.byref(s), C.byref(o),
+                                               C.byref(st)), "vsg_search_exact_command")
+        return {k: getattr(st, k) for k, _ in SearchExactStats._fields_}
+
     def udb_load(self, udb: "Udb"):
         """vsg_udb_load: (SeqSetHandle, IndexHandle, mask_lower) of a parsed UDB file"""
         sh = C.c_void_p(); ih = C.c_void_p(); ml = C.c_int(-1)
@@ -841,4 +866,49 @@ def cluster_write(headers, seqs, abundances, results: np.ndarray, cigars, uc: Op
     return int(single.value)
 
 
+class ExactIndex:
+    """vsg_exact_index handle"""
 
+    def __init__(self, h):
+        self.h = h
+
+    def close(self):
+        if self.h:
+            load().vsg_exact_index_destroy(self.h)
+            self.h = None
+
+
+class SearchExactOpts(C.Structure):
+    _fields_ = [("dbmask", C.c_int32), ("qmask", C.c_int32), ("hardmask", C.c_int32), ("sizein", C.c_int32),
+                ("sizeout", C.c_int32), ("xsize", C.c_int32), ("notrunclabels", C.c_int32), ("fasta_width", C.c_int32),
+                ("minseqlength", C.c_int64), ("maxseqlength", C.c_int64), ("maxhits", C.c_int64), ("uc_allhits", C.c_int32),
+                ("output_no_hits", C.c_int32), ("batch_queries", C.c_int32), ("reserved", C.c_int32)]
+
+
+SEARCH_EXACT_OUTPUTS = ("blast6out", "uc", "matched", "notmatched", "dbmatched", "dbnotmatched", "otutabout", "mothur_shared_out")
+
+
+class SearchExactOutputs(C.Structure):
+    _fields_ = [(k, C.c_char_p) for k in SEARCH_EXACT_OUTPUTS]
+
+
+class SearchExactStats(C.Structure):
+    _fields_ = [("queries", C.c_int64), ("matched", C.c_int64), ("queries_abundance", C.c_int64), ("matched_abundance", C.c_int64),
+                ("db_sequences", C.c_int64), ("db_discarded_short", C.c_int64), ("db_discarded_long", C.c_int64), ("hits", C.c_int64),
+                ("parse_s", C.c_double), ("device_s", C.c_double), ("write_s", C.c_double), ("wall_s", C.c_double)]
+
+
+def search_exact_opts(**kw):
+    """vsg_search_exact_opts_default, then the given fields: output paths into SearchExactOutputs, the fields of
+    vsg_search_exact_opts there, the rest into the search options.  Returns (SearchExactOpts, SearchOpts, SearchExactOutputs)."""
+    e, s, o = SearchExactOpts(), SearchOpts(), SearchExactOutputs()
+    load().vsg_search_exact_opts_default(C.byref(e), C.byref(s))
+    names = {k for k, _ in SearchExactOpts._fields_}
+    for k, v in kw.items():
+        if k in SEARCH_EXACT_OUTPUTS:
+            setattr(o, k, v.encode() if isinstance(v, str) else v)
+        elif k in names:
+            setattr(e, k, int(DBMASK[v] if isinstance(v, str) else v))
+        else:
+            setattr(s, k, v)
+    return e, s, o
