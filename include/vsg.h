@@ -705,6 +705,73 @@ void vsg_search_exact_opts_default(vsg_search_exact_opts * e, vsg_search_opts * 
 int vsg_search_exact_command(vsg_ctx * ctx, const char * query_path, const char * db_path, const vsg_search_exact_opts * e,
                              const vsg_search_opts * s, const vsg_search_exact_outputs * outputs, vsg_search_exact_stats * stats);
 
+/* ---- the --usearch_global command: replaces usearch_global() (commands/usearch_global.cpp:150-373, 537-845) on one
+ *      context (one GPU).  The database: a UDB file (vsg_udb_detect) is read by vsg_udb_open / vsg_udb_load, its mask and
+ *      word length are the file's, its headers and sequences are printed as stored; any other file is read whole as db.read
+ *      keeps it (FASTA or FASTQ, labels cut at the first blank unless notrunclabels, records outside [minseqlength,
+ *      maxseqlength] discarded and counted), with dbmask dust DUST-masked on the device, with soft + hardmask lower case
+ *      turned into 'N', and indexed at s->wordlength with lower case out of the words unless dbmask is none.  Abundances
+ *      come from ";size=".  Queries (FASTA or FASTQ) stream in batches of batch_queries over a reader thread, the device
+ *      and a writer thread, rows in input order (the reference's order with --threads 1).  Per batch on the device: upload,
+ *      qmask (dust: vsg_seqset_dust, the minus strand masked on its own; soft + hardmask: 'N' on the host), the search with
+ *      every hit kept (vsg_search_hits with maxhits 0, query_sizes from ";size=", --self label identities), then the CIGAR
+ *      of every --uc row that is printed and is not "=" (vsg_align_pairs: plus-strand rows against the searched query set,
+ *      minus-strand rows against its vsg_seqset_revcomp).  The writer is vsg_search_write's.  A query whose only hits are
+ *      weak (weak_id below id) is matched, as search_joinhits keeps it.  Refused with VSG_EINVAL and no file left: no
+ *      output, gzip or bzip2 input, qmask or dbmask dust with hardmask, a missing file, negative maxhits, non-NULL size or
+ *      label arrays in s, and a --uc row whose alignment the 16-bit aligner defers (its CIGAR cannot come from the
+ *      fallback callback).  Not offered: --alnout, --samout, --userout, --fastapairs, --qsegout, --tsegout, --lcaout,
+ *      --biomout, --relabel*, --label_suffix, --sample, several GPUs (vsg_usearch_stream is the multi-GPU --blast6out
+ *      stream).  s carries id, weak_id, maxaccepts, maxrejects, wordlength, strand_both and the filters; its size and label
+ *      arrays are the command's own (pass them NULL).  vsg_usearch_global_opts_default fills the CLI's defaults (cli.cc):
+ *      dbmask and qmask dust, minseqlength 32, maxseqlength 50 000, fasta_width 80, maxhits 0 (all), batch_queries 65 536,
+ *      and vsg_search_opts_default's (maxaccepts 1, maxrejects 32, wordlength 8); the caller sets id.
+ *      vsg_search_write needs no device: the output files of nq queries (headers as kept, sequences as printed, i.e. as
+ *      masked, abundances) with their search rows (query i's are rows[first[i] .. first[i + 1]), every hit, in
+ *      search_joinhits order) against ndb database records (headers, sequences as printed, abundances).  cigar_off[j]
+ *      (one per row) places row j's NUL-terminated CIGAR in cigar_buf; it is read only for a printed --uc row whose matches
+ *      differ from its alignment length.  --blast6out: at most maxhits rows per query (the "*" row with output_no_hits);
+ *      --uc: an H row for the first of them (every one with uc_allhits; column 2 the target number, column 3 the query
+ *      length, "=" when matches == alignment length, terminal gaps included, else the CIGAR), an N row for a query without
+ *      hits; top_hits_only stops both at the first row whose id is below the first row's.  --matched / --notmatched: the
+ *      queries with / without a hit.  --otutabout / --mothur_shared_out: each query's first row's target (core/otutable.cpp,
+ *      as for --search_exact), unmatched targets added with 0.  --dbmatched: the targets of any row, abundance the query
+ *      abundances summed with sizein, the row count without; --dbnotmatched: the others with their own abundance.
+ *      *matched (optional): the queries with a hit.  A failed write leaves no file. ---- */
+typedef struct vsg_usearch_global_opts {
+  int32_t dbmask;           /* --dbmask: VSG_DBMASK_NONE / _SOFT / _DUST (default dust); ignored for a UDB database */
+  int32_t qmask;            /* --qmask (default dust) */
+  int32_t hardmask;         /* --hardmask (with soft: lower case becomes 'N'; refused with dust) */
+  int32_t sizein;           /* --sizein: --dbmatched abundances sum the query abundances */
+  int32_t sizeout;          /* --sizeout */
+  int32_t xsize;            /* --xsize */
+  int32_t notrunclabels;    /* --notrunclabels */
+  int32_t fasta_width;      /* --fasta_width (default 80; 0: one line) */
+  int64_t minseqlength;     /* --minseqlength (default 32) */
+  int64_t maxseqlength;     /* --maxseqlength (default 50 000) */
+  int64_t maxhits;          /* --maxhits (0: all) */
+  int32_t uc_allhits;       /* --uc_allhits */
+  int32_t output_no_hits;   /* --output_no_hits */
+  int32_t top_hits_only;    /* --top_hits_only */
+  int32_t batch_queries;    /* queries per device call (default 65 536) */
+} vsg_usearch_global_opts;
+typedef vsg_search_exact_outputs vsg_usearch_global_outputs;
+typedef struct vsg_usearch_global_stats {
+  int64_t queries, matched;                     /* "Matching unique query sequences: matched of queries" */
+  int64_t queries_abundance, matched_abundance; /* "Matching total query sequences" (printed with --sizein) */
+  int64_t db_sequences, db_discarded_short, db_discarded_long, hits;
+  int64_t pairs, cells;                         /* the search's alignments and their DP cells */
+  double parse_s, device_s, cigar_s, write_s, wall_s;
+} vsg_usearch_global_stats;
+void vsg_usearch_global_opts_default(vsg_usearch_global_opts * u, vsg_search_opts * s);
+int vsg_usearch_global_command(vsg_ctx * ctx, const char * query_path, const char * db_path, const vsg_usearch_global_opts * u,
+                               const vsg_search_opts * s, const vsg_usearch_global_outputs * outputs, vsg_usearch_global_stats * stats);
+int vsg_search_write(int64_t nq, const char * const * query_headers, const char * qcat, const int64_t * qoff, const int32_t * qlen,
+                     const int64_t * query_sizes, const vsg_search_result * rows, const int64_t * first, const char * cigar_buf,
+                     const int64_t * cigar_off, int64_t ndb, const char * const * db_headers, const char * dbcat,
+                     const int64_t * dboff, const int32_t * dblen, const int64_t * db_sizes, const vsg_usearch_global_opts * u,
+                     const vsg_usearch_global_outputs * outputs, int64_t * matched);
+
 #ifdef __cplusplus
 }
 #endif

@@ -382,38 +382,24 @@ extern "C" int vsg_cluster_command(vsg_ctx * ctx, const char * input_path, const
 
     // the CIGARs of the H records: plus-strand members against the set, minus-strand ones as reverse complements
     auto const t_cigar = std::chrono::steady_clock::now();
-    SeqsetPtr rc_set;
-    for (int strand = 0; strand < 2; strand++) {
-      std::vector<uint32_t> q, t;
-      int64_t cap = 0;
-      for (int64_t k = 0; k < n; k++) {
-        vsg_cluster_result const & r = res[static_cast<size_t>(k)];
-        if (r.centroid < 0 || r.strand != strand) { continue; }
-        q.push_back(static_cast<uint32_t>(k));
-        t.push_back(static_cast<uint32_t>(r.centroid));
-        cap += len[static_cast<size_t>(k)] + len[static_cast<size_t>(r.centroid)] + 1;
-      }
-      if (q.empty()) { continue; }
-      if (strand == 1 && (rc = seqset_revcomp(ctx, set.get(), 0, n, rc_set)) != VSG_OK) { return rc; }
-      size_t const m = q.size();
-      std::vector<int16_t> score(m);
-      std::vector<uint16_t> aligned(m), matches(m), mismatches(m), gaps(m);
-      std::vector<char> buf(static_cast<size_t>(cap) + 1);
-      std::vector<int64_t> bo(m + 1);
-      if ((rc = vsg_align_pairs(ctx, strand == 0 ? set.get() : rc_set.get(), set.get(), static_cast<int64_t>(m), q.data(), t.data(),
-                                score.data(), aligned.data(), matches.data(), mismatches.data(), gaps.data(), nullptr, buf.data(),
-                                cap + 1, bo.data())) != VSG_OK) { return rc; }
-      for (size_t j = 0; j < m; j++) {
-        if (score[j] == VSG_SCORE_SENTINEL) {
-          Error::set(std::string("vsg_cluster_command: the 16-bit aligner defers the alignment of ") + heads[q[j]] + " with its centroid " +
-                     heads[t[j]] + ": its CIGAR for --uc cannot come from the fallback callback");
-          return VSG_EINVAL;
-        }
-        cigar_off[q[j]] = static_cast<int64_t>(cigars.size());
-        cigars.insert(cigars.end(), buf.begin() + bo[j], buf.begin() + bo[j + 1]);
-        if (cigars.back() != '\0') { cigars.push_back('\0'); }
-      }
+    std::vector<uint32_t> q, t;
+    std::vector<uint8_t> strand;
+    for (int64_t k = 0; k < n; k++) {
+      vsg_cluster_result const & r = res[static_cast<size_t>(k)];
+      if (r.centroid < 0) { continue; }
+      q.push_back(static_cast<uint32_t>(k));
+      t.push_back(static_cast<uint32_t>(r.centroid));
+      strand.push_back(r.strand != 0 ? 1 : 0);
     }
+    std::vector<int64_t> offs;
+    int64_t deferred = -1;
+    if (!q.empty() && (rc = strand_cigars(ctx, set.get(), set.get(), q, t, strand, cigars, offs, deferred)) != VSG_OK) { return rc; }
+    if (deferred >= 0) {
+      Error::set(std::string("vsg_cluster_command: the 16-bit aligner defers the alignment of ") + heads[q[static_cast<size_t>(deferred)]] +
+                 " with its centroid " + heads[t[static_cast<size_t>(deferred)]] + ": its CIGAR for --uc cannot come from the fallback callback");
+      return VSG_EINVAL;
+    }
+    for (size_t j = 0; j < q.size(); j++) { cigar_off[q[j]] = offs[j]; }
     // the printed case is the device's (DUST), the letters the input's: 'U' and IUPAC codes print as read
     if (c->qmask == VSG_DBMASK_DUST) {
       std::vector<uint8_t> sym(cat.size());

@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <memory>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/vsg.h"
@@ -262,6 +263,94 @@ using SeqsetPtr = std::unique_ptr<vsg_seqset, SeqsetDeleter>;
 int seqset_revcomp(vsg_ctx * c, const vsg_seqset * src, int64_t q0, int64_t n, SeqsetPtr & out);
 // both strands of every sequence of src, sequence s at 2s and its reverse complement at 2s+1
 int seqset_both_strands(vsg_ctx * c, const vsg_seqset * src, SeqsetPtr & out);
+
+// ---- what the search commands share (search_out.cu) ----
+// DUST on the device, then the printed sequences `cat` (the set's, plus a NUL) take the device's case: dust_core
+// upper-cases, then lowers the masked symbols; the letters stay the input's
+int dust_case(vsg_ctx * ctx, vsg_seqset * set, std::vector<char> & cat);
+// --hardmask with --qmask / --dbmask soft (hardmask / hardmask_all, core/mask.cpp): lower case becomes 'N'
+void hardmask(std::vector<char> & cat);
+// A search command's database: the records as printed (file), their abundances from ";size=", the header pointers, the
+// device set as searched and, for --self, label identities (label_id[t] = the first record with t's header).
+struct SearchDb {
+  FastxFile file;
+  std::vector<int64_t> size;
+  std::vector<const char *> heads;
+  SeqsetPtr set;
+  std::vector<int64_t> label_id;
+  std::unordered_map<std::string, int64_t> label_ids;
+};
+// size, heads and (self) the label identities of db.file's records
+int search_db_labels(const char * caller, bool self, SearchDb & db);
+// db.read(..., upcase = 0) under [minlen, maxlen], lower case to 'N' for dbmask soft + hardmask, search_db_labels, the
+// device set, and with `dust` DUST on the device with the printed case (dust_case)
+int search_db_read(vsg_ctx * ctx, const char * caller, const char * path, bool notrunclabels, int64_t minlen, int64_t maxlen,
+                   int dbmask, bool hardmask_soft, bool dust, bool self, SearchDb & db);
+// o = s with a batch's query abundances (from heads' ";size="), the database's, and for --self the queries' label identities
+int search_batch_opts(const char * caller, const std::vector<std::string> & heads, const SearchDb & db, const vsg_search_opts & s,
+                      std::vector<int64_t> & size, std::vector<int64_t> & label, vsg_search_opts & o);
+
+// The output files of a search command (search_output_results and the end of usearch_global / search_exact): fed
+// batches of queries with their rows in input order (batch), then the end-of-run files (finish).  Where the two commands
+// differ is a parameter.
+struct SearchWriterOpts {
+  int64_t maxhits = 0;            // 0: all
+  bool top_hits_only = false, uc_allhits = false, output_no_hits = false, sizein = false, xsize = false;
+  bool weak_dbmatched = false;    // a weak hit marks its target too (usearch_global.cpp:368-372; search_exact: accepted only)
+  bool dbnotmatched_size = false; // --dbnotmatched prints the target's abundance (usearch_global.cpp:828), not 0 (search_exact)
+  FastaFormat fmt{nullptr, false, false, 80};
+};
+SearchWriterOpts usearch_global_writer_opts(const vsg_usearch_global_opts & u);
+// one batch: query i's rows are rows[first[i] .. first[i + 1]); a printed --uc row j that is not "=" reads its CIGAR at
+// cigar_buf + cigar_off[j]
+struct SearchRows {
+  int64_t nq;
+  const std::string * head;
+  const char * cat;
+  const int64_t * off;
+  const int32_t * len;
+  const int64_t * size;
+  const vsg_search_result * rows;
+  const int64_t * first;
+  const char * cigar_buf;
+  const int64_t * cigar_off;
+};
+struct OtuTable;
+class SearchWriter {
+ public:
+  SearchWriter(const SearchWriterOpts & o, const vsg_search_exact_outputs & out, const std::vector<std::string> & dbhead,
+               const char * dbcat, const int64_t * dboff, const int32_t * dblen, const int64_t * dbsize);
+  ~SearchWriter();
+  // the rows of a query's n hits that --blast6out / --uc show: min(maxhits, n), cut by --top_hits_only
+  int64_t shown(const vsg_search_result * r, int64_t n) const;
+  // of those, the rows --uc prints
+  int64_t uc_rows(int64_t shown) const;
+  // appends the batch's rows to outs[0..3] = blast6out, uc, matched, notmatched, and accumulates the rest
+  void batch(const SearchRows & b, std::string * outs);
+  // --otutabout, --mothur_shared_out, --dbmatched, --dbnotmatched through files; false (error set) on a failed write
+  bool finish(const char * caller, OutFiles & files);
+  int64_t queries = 0, matched = 0, queries_abundance = 0, matched_abundance = 0, hits = 0, blast6 = 0;
+ private:
+  const char * const * dbhead_ptrs();
+  SearchWriterOpts o_;
+  vsg_search_exact_outputs out_;
+  const std::vector<std::string> & dbhead_;
+  const char * dbcat_;
+  const int64_t * dboff_;
+  const int32_t * dblen_;
+  const int64_t * dbsize_;
+  std::vector<uint64_t> dbmatched_;
+  std::vector<const char *> dbheads_;
+  std::unique_ptr<OtuTable> otu_;
+};
+
+// The CIGARs of pairs (q[j], t[j]) on strand[j], two vsg_align_pairs calls: plus-strand pairs align queries' q against
+// targets' t, minus-strand pairs the reverse complement of queries' q (vsg_seqset_revcomp of the whole set).  Pair j's
+// NUL-terminated CIGAR is appended to buf at offs[j]; deferred = the first pair the 16-bit aligner defers
+// (VSG_SCORE_SENTINEL; its offs stays -1), or -1.
+int strand_cigars(vsg_ctx * c, const vsg_seqset * queries, const vsg_seqset * targets, const std::vector<uint32_t> & q,
+                  const std::vector<uint32_t> & t, const std::vector<uint8_t> & strand, std::vector<char> & buf,
+                  std::vector<int64_t> & offs, int64_t & deferred);
 
 }  // namespace vsg
 

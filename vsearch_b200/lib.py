@@ -406,6 +406,17 @@ class Context:
                                                C.byref(st)), "vsg_search_exact_command")
         return {k: getattr(st, k) for k, _ in SearchExactStats._fields_}
 
+    def usearch_global_command(self, query_path: str, db_path: str, /, **kw) -> dict:
+        """vsg_usearch_global_command (--usearch_global): keywords naming an output of SearchExactOutputs give its path,
+        those of vsg_usearch_global_opts its value (qmask / dbmask may be "none" / "soft" / "dust"), the rest go to the
+        search options (id, weak_id, maxaccepts, strand_both, self, ...; the arguments before them are positional-only, so
+        `self` can be one).  db_path may be a FASTA / FASTQ file or a UDB file.  Returns the stats as a dict."""
+        u, s, o = usearch_global_opts(**kw)
+        st = UsearchGlobalStats()
+        _check(load().vsg_usearch_global_command(self.h, query_path.encode(), db_path.encode(), C.byref(u), C.byref(s), C.byref(o),
+                                                 C.byref(st)), "vsg_usearch_global_command")
+        return {k: getattr(st, k) for k, _ in UsearchGlobalStats._fields_}
+
     def udb_load(self, udb: "Udb"):
         """vsg_udb_load: (SeqSetHandle, IndexHandle, mask_lower) of a parsed UDB file"""
         sh = C.c_void_p(); ih = C.c_void_p(); ml = C.c_int(-1)
@@ -912,3 +923,74 @@ def search_exact_opts(**kw):
         else:
             setattr(s, k, v)
     return e, s, o
+
+
+class UsearchGlobalOpts(C.Structure):
+    _fields_ = [("dbmask", C.c_int32), ("qmask", C.c_int32), ("hardmask", C.c_int32), ("sizein", C.c_int32),
+                ("sizeout", C.c_int32), ("xsize", C.c_int32), ("notrunclabels", C.c_int32), ("fasta_width", C.c_int32),
+                ("minseqlength", C.c_int64), ("maxseqlength", C.c_int64), ("maxhits", C.c_int64), ("uc_allhits", C.c_int32),
+                ("output_no_hits", C.c_int32), ("top_hits_only", C.c_int32), ("batch_queries", C.c_int32)]
+
+
+class UsearchGlobalStats(C.Structure):
+    _fields_ = [("queries", C.c_int64), ("matched", C.c_int64), ("queries_abundance", C.c_int64), ("matched_abundance", C.c_int64),
+                ("db_sequences", C.c_int64), ("db_discarded_short", C.c_int64), ("db_discarded_long", C.c_int64), ("hits", C.c_int64),
+                ("pairs", C.c_int64), ("cells", C.c_int64), ("parse_s", C.c_double), ("device_s", C.c_double),
+                ("cigar_s", C.c_double), ("write_s", C.c_double), ("wall_s", C.c_double)]
+
+
+def usearch_global_opts(**kw):
+    """vsg_usearch_global_opts_default, then the given fields: output paths into SearchExactOutputs, the fields of
+    vsg_usearch_global_opts there, the rest into the search options.  Returns (UsearchGlobalOpts, SearchOpts,
+    SearchExactOutputs)."""
+    u, s, o = UsearchGlobalOpts(), SearchOpts(), SearchExactOutputs()
+    load().vsg_usearch_global_opts_default(C.byref(u), C.byref(s))
+    names = {k for k, _ in UsearchGlobalOpts._fields_}
+    for k, v in kw.items():
+        if k in SEARCH_EXACT_OUTPUTS:
+            setattr(o, k, v.encode() if isinstance(v, str) else v)
+        elif k in names:
+            setattr(u, k, int(DBMASK[v] if isinstance(v, str) else v))
+        else:
+            setattr(s, k, v)
+    return u, s, o
+
+
+def _packed(seqs):
+    """(cat, off, len) arrays of a list of bytes"""
+    cat = np.frombuffer(b"".join(seqs) + b"\0", dtype=np.uint8)
+    ln = np.array([len(x) for x in seqs], dtype=np.int32)
+    off = np.zeros(max(len(seqs), 1), dtype=np.int64)
+    if len(seqs) > 1:
+        off[1:len(seqs)] = np.cumsum(ln[:-1], dtype=np.int64)
+    return cat, off, ln
+
+
+def search_write(query_headers, query_seqs, query_sizes, hits, db_headers, db_seqs, db_sizes, **kw) -> int:
+    """vsg_search_write (host only, no device): the --usearch_global output files of one batch of queries.  hits[i] is
+    query i's list of (SearchResult, CIGAR str, or None for none) in search_joinhits order; sequences are bytes as printed; kw as
+    usearch_global_command (output paths and vsg_usearch_global_opts fields).  Returns the number of matched queries."""
+    u, _, o = usearch_global_opts(**kw)
+    nq, ndb = len(query_headers), len(db_headers)
+    first = np.zeros(nq + 1, dtype=np.int64)
+    first[1:] = np.cumsum([len(h) for h in hits], dtype=np.int64) if nq else []
+    flat = [h for hs in hits for h in hs]
+    rows = (SearchResult * max(len(flat), 1))(*[r for r, _ in flat])
+    cig = [(c or "").encode() + b"\0" for _, c in flat]
+    cbuf = np.frombuffer(b"".join(cig) + b"\0", dtype=np.uint8)
+    coff = np.zeros(max(len(flat), 1), dtype=np.int64)
+    if len(flat) > 1:
+        coff[1:len(flat)] = np.cumsum([len(x) for x in cig[:-1]], dtype=np.int64)
+    coff[[j for j, (_, c) in enumerate(flat) if c is None]] = -1   # no CIGAR
+    qcat, qoff, qlen = _packed(query_seqs)
+    dcat, doff, dlen = _packed(db_seqs)
+    qs = np.ascontiguousarray(query_sizes, dtype=np.int64)
+    ds = np.ascontiguousarray(db_sizes, dtype=np.int64)
+    matched = C.c_int64()
+    _check(load().vsg_search_write(C.c_int64(nq), _strings(query_headers) if nq else None, qcat.ctypes.data_as(C.c_char_p),
+                                   _ptr(qoff, C.c_int64), _ptr(qlen, C.c_int32), _ptr(qs, C.c_int64), rows, _ptr(first, C.c_int64),
+                                   cbuf.ctypes.data_as(C.c_char_p), _ptr(coff, C.c_int64), C.c_int64(ndb),
+                                   _strings(db_headers) if ndb else None, dcat.ctypes.data_as(C.c_char_p), _ptr(doff, C.c_int64),
+                                   _ptr(dlen, C.c_int32), _ptr(ds, C.c_int64), C.byref(u), C.byref(o), C.byref(matched)),
+           "vsg_search_write")
+    return int(matched.value)
