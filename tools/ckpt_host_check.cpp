@@ -102,6 +102,35 @@ static int forward(const Score & sp, const std::vector<uint8_t> & q, const std::
   return score;
 }
 
+// fast_path_ok (vsg_api.cu): every intermediate of a (qpad x d) problem stays inside the 16-bit range
+static bool path_ok(const Score & p, int qpad, int d)
+{
+  int64_t G = 0, Rm = 0, smax = 0, smin = 0;
+  for (int k = 0; k < 6; k++) {
+    if (p.go[k] < 0 || p.ge[k] < 0) { return false; }
+    G = std::max<int64_t>(G, p.go[k] + p.ge[k]);
+    Rm = std::max<int64_t>(Rm, p.ge[k]);
+  }
+  for (int i = 0; i < 16; i++) {
+    for (int j = 0; j < 16; j++) { smax = std::max<int64_t>(smax, p.S[i][j]); smin = std::min<int64_t>(smin, p.S[i][j]); }
+  }
+  int64_t const lb = -(G + static_cast<int64_t>(qpad) * Rm) - G - static_cast<int64_t>(d + 4) * Rm - 2 * G + smin;
+  int64_t const ub = smax * std::min<int64_t>(qpad, d + 4) + smax;
+  return lb > -32700 && ub < 32700;
+}
+
+// the longest target (at most cap) the planner sends to the checkpoint kernels with R rows per lane: inside the
+// bound of the scoring and of its shift (plan_pairs); 0 when there is none
+static int ckpt_bound(const Score & p0, const Score & p, int R, int cap)
+{
+  int d = 0;
+  for (int step = 1 << 16; step > 0; step >>= 1) {
+    int const t = d + step;
+    if (t <= cap && path_ok(p0, 32 * R, t) && path_ok(p, 32 * R, t)) { d = t; }
+  }
+  return d;
+}
+
 static std::string cigar_of(const std::string & rev)
 {
   std::string out;
@@ -120,33 +149,73 @@ static std::string cigar_of(const std::string & rev)
 int main(int argc, char ** argv)
 {
   int const n = argc > 1 ? std::atoi(argv[1]) : 400;
+  std::string const mode = argc > 3 ? argv[3] : "mixed";
+  int const longest = argc > 2 ? std::atoi(argv[2]) : (mode == "mixed" ? 300 : 65535);
+  if ((mode != "mixed" && mode != "long" && mode != "limits") || longest < 1) {
+    std::fprintf(stderr, "usage: ckpt_host_check [cases [longest target [mixed|long|limits]]]\n");
+    return 2;
+  }
   std::mt19937 rng(12345);
   const char * acgt = "ACGT";
   const char * iupac = "ACGTUNRYSWKMBDHVacgtn";
-  int bad = 0, checked = 0;
+  int bad = 0, checked = 0, longest_seen = 0, shifted_min = 0, score_max = 0;
   for (int k = 0; k < n; k++) {
     oracle_scoring sc;
     oracle_default_scoring(&sc);
-    if (k % 3 == 2) {
+    if (mode == "mixed" && k % 3 == 2) {
       sc.v[0] = 1 + rng() % 4; sc.v[1] = -static_cast<int64_t>(1 + rng() % 6);
       for (int z = 0; z < 6; z++) { sc.v[2 + z] = rng() % 22; sc.v[8 + z] = rng() % 4; }
     }
-    sc.n_mismatch = (k % 7 == 6);
+    if (mode == "limits") {
+      if (k % 3 == 0) {
+        sc.v[0] = 2; sc.v[1] = -80;
+        for (int z = 0; z < 6; z++) { sc.v[2 + z] = 20; sc.v[8 + z] = 40; }
+      } else {
+        sc.v[0] = k % 3 == 1 ? 60 : 64; sc.v[1] = -4;
+      }
+    }
+    sc.n_mismatch = mode != "limits" && (k % 7 == 6);
     Score sp0; build(sc, sp0);
     Score const sp = shifted(sp0);
-    const char * A = (k % 5 == 4) ? iupac : acgt;
+    const char * A = (mode != "limits" && k % 5 == 4) ? iupac : acgt;
     size_t const na = std::strlen(A);
     int const R = 1 + rng() % 16;
-    int const Q = 1 + rng() % (32 * R);            // single strip
+    int const Q = mode == "limits" ? 32 * R : 1 + static_cast<int>(rng() % (32 * R));   // single strip
     std::string qs(Q, 'A');
     for (auto & ch : qs) { ch = A[rng() % na]; }
     std::string ts[2];
-    for (int h = 0; h < 2; h++) {
-      int const D = 1 + rng() % 300;
-      ts[h].assign(D, 'A');
-      for (int x = 0; x < D; x++) { ts[h][x] = (k % 2 == 0 && x < Q && rng() % 10 != 0) ? qs[x] : A[rng() % na]; }
+    if (mode == "mixed") {
+      for (int h = 0; h < 2; h++) {
+        int const D = 1 + rng() % longest;
+        ts[h].assign(D, 'A');
+        for (int x = 0; x < D; x++) { ts[h][x] = (k % 2 == 0 && x < Q && rng() % 10 != 0) ? qs[x] : A[rng() % na]; }
+      }
+    } else {
+      int const dck = ckpt_bound(sp0, sp, R, longest);
+      if (dck < 1) { continue; }
+      for (int h = 0; h < 2; h++) {
+        int D = dck - static_cast<int>(rng() % 3);
+        if (mode == "long" && h == 1 && k % 3 == 0) { D = 1 + rng() % 64; }
+        D = std::max(D, 1);
+        // a relative of the query: 5 % substitutions
+        std::string m = qs;
+        for (auto & ch : m) { if (rng() % 20 == 0) { ch = A[rng() % na]; } }
+        std::string t(D, 'A');
+        for (auto & ch : t) { ch = A[rng() % na]; }
+        bool const unrelated = mode == "limits" && k % 3 == 0;   // harsh penalties: the lowest scores
+        if (!unrelated) {
+          if (D <= Q) { t = m.substr(static_cast<size_t>(rng() % (Q - D + 1)), static_cast<size_t>(D)); }
+          else {
+            int const where = (k + h) % 3;   // 0: query at the start, 1: at the end, 2: in the middle
+            int const at = where == 0 ? 0 : (where == 1 ? D - Q : (D - Q) / 2);
+            t.replace(static_cast<size_t>(at), static_cast<size_t>(Q), m);
+          }
+        }
+        ts[h] = t;
+      }
     }
     int const dmax = static_cast<int>(std::max(ts[0].size(), ts[1].size()));
+    longest_seen = std::max(longest_seen, dmax);
     std::vector<U2> rowck(row_elems(dmax), U2{0xdeaddeadu, 0xdeaddeadu});
     std::vector<U2> colck(col_elems(dmax, R), U2{0xdeaddeadu, 0xdeaddeadu});
     std::vector<uint8_t> q4(Q);
@@ -158,6 +227,7 @@ int main(int argc, char ** argv)
       int const score = forward(sp, q4, t4, R, h, rowck, colck);
       // (the second target's forward pass runs before the first one's traceback in a kernel too)
       if (h == 0) { continue; }
+      shifted_min = std::min(shifted_min, score);
       for (int hh = 0; hh < 2; hh++) {
         int const DD = static_cast<int>(ts[hh].size());
         std::vector<uint8_t> tt(DD);
@@ -178,6 +248,7 @@ int main(int argc, char ** argv)
         if (oracle_nw16(&sc, qs.data(), Q, ts[hh].data(), DD, &os, &oa, &om, &omi, &og, cig.data(), cig.size()) != 0) { std::fprintf(stderr, "oracle_nw16 failed\n"); return 2; }
         if (os == ORACLE_SENTINEL) { continue; }
         checked++;
+        score_max = std::max<int>(score_max, os);
         std::string const got = cigar_of(rev);
         bool ok = got == cig.data() && out.aligned == oa && out.matches == om && out.mismatches == omi && out.gaps == og;
         {
@@ -209,6 +280,7 @@ int main(int argc, char ** argv)
       }
     }
   }
-  std::printf("%d pairs checked, %d mismatches\n", checked, bad);
+  std::printf("%d pairs checked, %d mismatches (longest target %d, lowest shifted score %d, highest score %d)\n", checked, bad,
+              longest_seen, shifted_min, score_max);
   return bad != 0;
 }
