@@ -580,8 +580,9 @@ int vsg_orient_stream(vsg_group * g, const char * query_path, int query_mask_low
  *      device's case (the DUST mask).  Then vsg_cluster_write.  Refused with VSG_EINVAL and no output file: compressed
  *      input, --qmask dust --hardmask, a word length outside 3..10, an unsorted _SMALLMEM input without usersort, and a
  *      pair the 16-bit aligner defers (its CIGAR cannot come from the fallback callback).  Not offered: --alnout,
- *      --samout, --userout, --blast6out, --matched, --notmatched, OTU tables, --msaout, --consout, --profile,
+ *      --samout, --userout, --blast6out, --matched, --notmatched, OTU tables,
  *      --relabel_sha1 / _md5 / _self, --label_suffix, --sample, several GPUs.  The reference's stderr summary is `stats`.
+ *      (--msaout, --consout and --profile: vsg_cluster_command_outputs, below.)
  *      vsg_cluster_cmd_opts_default fills each command's CLI defaults (cli.cc): maxrejects 8 for --cluster_fast and 32
  *      otherwise, weak_id 0.90, minsize 8 and id -1 (not given) for --cluster_unoise, minseqlength 32, maxseqlength 50 000,
  *      wordlength 8, qmask dust, fasta_width 80; the caller sets id and whatever else the user gave.
@@ -630,6 +631,52 @@ int vsg_cluster_write(int64_t n, const char * const * headers, const char * cat,
                       const int64_t * abundances, const vsg_cluster_result * results, const char * cigar_buf,
                       const int64_t * cigar_off, const vsg_cluster_cmd_opts * c, const char * uc, const char * centroids,
                       const char * clusters_prefix, int64_t * singletons);
+
+/* ---- cluster consensus: replaces msa() (core/msa.cpp) as cluster() calls it for --msaout, --consout and --profile
+ *      (core/cluster.cpp:1473-1539).  vsg_cluster_msa takes the n records of `set` in processing order (the set as
+ *      clustered and masked: vsg_cluster_command's, or the one given to vsg_cluster_fast or a cluster session), their
+ *      vsg_cluster_result, their weights (the abundance with --sizein, else 1; at least 1) and the CIGAR of every H record
+ *      (cigar_buf + cigar_off[i], NUL-terminated, as vsg_cluster_write takes them; the member, reverse-complemented on
+ *      strand 1, against its centroid).  Per cluster, in cluster-number order, the rows are the centroid then the members
+ *      in processing order.  insertions: the widths of the len(centroid) + 1 insertion blocks of every cluster, back to
+ *      back (sum of len(centroid) + 1 entries; block p comes before centroid symbol p, the last after the centroid; its
+ *      width is the longest D run at p, find_max_insertions_per_position).  col_first: nclusters + 1 entries, cluster c's
+ *      columns are [col_first[c], col_first[c + 1]).  profile: 6 counters per column, A, C, G, T / U, N (every other IUPAC
+ *      code), gap, each the sum of the weights of the rows with that symbol in the column (upper case, minus-strand rows
+ *      complemented).  consensus: one char per column, the consensus row --msaout prints: '+' in the first insertions[0]
+ *      and last insertions[len] columns of the cluster, else the best of A, C, G, T (a tie goes to the first), or N when
+ *      none of them occurs and N does, if its count reaches the gaps, otherwise '-'.  *ncolumns receives the number of
+ *      columns; above cap the call returns VSG_ECAP with insertions and col_first filled, profile and consensus untouched.
+ *      The device work runs in chunks of whole clusters under a quarter of the context's direction-bit budget
+ *      (VSG_DIR_BUDGET_MB), at most 1 GiB; a cluster that needs more runs alone.  With VSG_TRACE the kernel time (CUDA
+ *      events) goes to stderr.
+ *      vsg_cluster_msa_write needs no device: the files of msa() for records as vsg_cluster_write takes them, with the
+ *      arrays of vsg_cluster_msa.  Clusters come in cluster-number order, with clusterout_sort by cluster abundance
+ *      descending first.  --msaout: per cluster an empty line, the centroid row under ">*" + its header, each member row
+ *      under its header (the record's own abundance for --sizeout; --relabel does not apply), ">consensus" and the
+ *      consensus row; rows print the sequences as given, minus-strand rows reverse-complemented with the reference's
+ *      complement map (case kept, U to A, anything else N); fasta_width applies.  --consout: the consensus without '+'
+ *      and '-' under "centroid=" + the centroid's header (fasta_print_general with --relabel <prefix><cluster + 1>,
+ *      ";seqs=<rows>", ";clusterid=" with clusterout_id, ";size=<cluster abundance>" with --sizeout).  --profile: that
+ *      header line alone, then per column "column\tconsensus symbol\tA\tC\tG\tT\tgap\tN" and an empty line.  Any path
+ *      may be NULL.  A failed write removes every file the call made. ---- */
+int vsg_cluster_msa(vsg_ctx * ctx, const vsg_seqset * set, int64_t n, const vsg_cluster_result * results, const uint64_t * weights,
+                    const char * cigar_buf, const int64_t * cigar_off, int32_t * insertions, int64_t * col_first, uint64_t * profile,
+                    char * consensus, int64_t cap, int64_t * ncolumns);
+int vsg_cluster_msa_write(int64_t n, const char * const * headers, const char * cat, const int64_t * off, const int32_t * len,
+                          const int64_t * abundances, const vsg_cluster_result * results, const char * cigar_buf,
+                          const int64_t * cigar_off, const int32_t * insertions, const int64_t * col_first, const uint64_t * profile,
+                          const char * consensus, const vsg_cluster_cmd_opts * c, const char * msaout, const char * consout,
+                          const char * profile_path);
+/* vsg_cluster_command_outputs: vsg_cluster_command with every output it offers; any path may be NULL.  With msaout,
+ *      consout or profile, after the CIGARs: vsg_cluster_msa (weights: the abundances with sizein, else 1) and
+ *      vsg_cluster_msa_write.  A failed call leaves none of the files it made.  vsg_cluster_command is this call with the
+ *      first three paths. */
+typedef struct vsg_cluster_cmd_outputs {
+  const char * uc, * centroids, * clusters_prefix, * msaout, * consout, * profile;
+} vsg_cluster_cmd_outputs;
+int vsg_cluster_command_outputs(vsg_ctx * ctx, const char * input_path, const vsg_cluster_cmd_opts * c, const vsg_search_opts * s,
+                                const vsg_cluster_cmd_outputs * outputs, vsg_cluster_cmd_stats * stats);
 
 /* ---- exact-match search: replaces Dbhash (core/dbhash.cpp) and search_exact_onequery / add_hit
  *      (commands/search_exact.cpp:136-209).  vsg_exact_index_create hashes every sequence of `db` on the device (the

@@ -507,19 +507,6 @@ extern "C" int vsg_sintax_stream(vsg_group * g, const char * const * target_head
 
 namespace {
 
-// reverse_complement (utils/reverse_complement.cpp) with the reference's complement map (utils/maps.cpp): IUPAC codes
-// to their complements in the same case, U to A, anything else to N
-struct Complement {
-  char map[256];
-  Complement()
-  {
-    std::memset(map, 'N', sizeof map);
-    char const * const from = "ACGTURYKMBVDHSWNacgturykmbvdhswn";
-    char const * const to = "TGCAAYRMKVBHDSWNtgcaayrmkvbhdswn";
-    for (int i = 0; from[i] != '\0'; i++) { map[static_cast<unsigned char>(from[i])] = to[i]; }
-  }
-};
-
 // fasta_print_general / fasta_print_sequence (core/fasta.cpp:423-450, 482-...) without header rewriting: lines of
 // `width` symbols (width < 1: one line, also for an empty sequence)
 void fasta_record(std::string & out, const std::string & head, const char * seq, int64_t len, int width)

@@ -229,13 +229,33 @@ struct FastaFormat {
   bool xsize, sizeout;
   int fasta_width;
 };
+// prefix: text before the label (NULL: none); seqs > 0: ";seqs=" (before ";clusterid="); seq NULL: no sequence line
 void fasta_print_general(std::string & out, const FastaFormat & f, const std::string & head, const char * seq, int64_t len,
-                         int64_t abundance, int64_t ordinal, int64_t clusterid);
+                         int64_t abundance, int64_t ordinal, int64_t clusterid, const char * prefix = nullptr, int64_t seqs = 0);
+// reverse_complement (utils/reverse_complement.cpp) with the reference's complement map (utils/maps.cpp): IUPAC codes
+// to their complements in the same case, U to A, anything else to N
+struct Complement {
+  char map[256];
+  Complement()
+  {
+    for (char & m : map) { m = 'N'; }
+    char const * const from = "ACGTURYKMBVDHSWNacgturykmbvdhswn";
+    char const * const to = "TGCAAYRMKVBHDSWNtgcaayrmkvbhdswn";
+    for (int i = 0; from[i] != '\0'; i++) { map[static_cast<unsigned char>(from[i])] = to[i]; }
+  }
+};
 // the files a call creates, removed again unless the call succeeds
 struct OutFiles {
   std::vector<std::string> made;
   bool ok = false;
   ~OutFiles() { if (!ok) { for (auto const & p : made) { std::remove(p.c_str()); } } }
+  // opens path for writing, to be removed again unless the call succeeds; NULL when it cannot be opened
+  std::FILE * open(const std::string & path)
+  {
+    std::FILE * f = std::fopen(path.c_str(), "wb");
+    if (f != nullptr) { made.push_back(path); }
+    return f;
+  }
   bool write(const std::string & path, const std::string & data)
   {
     std::FILE * f = std::fopen(path.c_str(), "wb");

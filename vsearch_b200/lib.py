@@ -371,15 +371,46 @@ class Context:
         return {k: getattr(st, k) for k, _ in MakeudbStats._fields_}
 
     def cluster_command(self, input_path: str, uc: Optional[str] = None, centroids: Optional[str] = None,
-                        clusters: Optional[str] = None, command: str = "cluster_fast", **opts) -> dict:
-        """vsg_cluster_command (--cluster_fast / _size / _smallmem / _unoise: a key of CLUSTER_COMMANDS): reads input_path,
-        writes --uc, --centroids and --clusters <prefix> (None: not written); opts as cluster_cmd_opts (id=0.97,
-        threads=8, qmask="soft", sizeout=1, ...).  Returns the stats as a dict."""
+                        clusters: Optional[str] = None, command: str = "cluster_fast", msaout: Optional[str] = None,
+                        consout: Optional[str] = None, profile: Optional[str] = None, **opts) -> dict:
+        """vsg_cluster_command_outputs (--cluster_fast / _size / _smallmem / _unoise: a key of CLUSTER_COMMANDS): reads
+        input_path, writes --uc, --centroids, --clusters <prefix>, --msaout, --consout and --profile (None: not written);
+        opts as cluster_cmd_opts (id=0.97, threads=8, qmask="soft", sizeout=1, ...).  Returns the stats as a dict."""
         c, s = cluster_cmd_opts(command, **opts)
         st = ClusterCmdStats()
-        _check(load().vsg_cluster_command(self.h, input_path.encode(), C.byref(c), C.byref(s),
-                                          *_cluster_cmd_paths(uc, centroids, clusters), C.byref(st)), "vsg_cluster_command")
+        out = ClusterCmdOutputs(*_cluster_cmd_paths(uc, centroids, clusters), *_cluster_cmd_paths(msaout, consout, profile))
+        _check(load().vsg_cluster_command_outputs(self.h, input_path.encode(), C.byref(c), C.byref(s), C.byref(out),
+                                                  C.byref(st)), "vsg_cluster_command")
         return {k: getattr(st, k) for k, _ in ClusterCmdStats._fields_}
+
+    def cluster_msa(self, ss: SeqSetHandle, results: np.ndarray, weights, cigars) -> dict:
+        """vsg_cluster_msa: the column layout, profile and consensus of the clusters of `results` (records of `ss` in
+        processing order, a cluster result array) with per-record `weights` and the CIGAR (str) of each H record.
+        Returns numpy arrays: insertions (int32), col_first (int64, clusters + 1), profile (uint64, columns x 6: A, C, G,
+        T, N, gap) and consensus (uint8, one char per column)."""
+        res = np.ascontiguousarray(results, dtype=_CLUSTER_DT)
+        n = res.shape[0]
+        w = np.ascontiguousarray(weights, dtype=np.uint64)
+        cbuf, coff = _cigar_buf(cigars, n)
+        nins = int((ss.lens[:n][res["centroid"] < 0].astype(np.int64) + 1).sum()) if n else 0
+        nclusters = int(res["cluster"].max()) + 1 if n else 0
+        ins = np.zeros(max(nins, 1), dtype=np.int32)
+        first = np.zeros(nclusters + 1, dtype=np.int64)
+        ncols = C.c_int64()
+        args = lambda prof, cons, cap: (self.h, ss.h, C.c_int64(n), res.ctypes.data_as(C.POINTER(ClusterResult)),  # noqa: E731
+                                        _ptr(w, C.c_uint64), cbuf.ctypes.data_as(C.c_char_p), _ptr(coff, C.c_int64),
+                                        _ptr(ins, C.c_int32), _ptr(first, C.c_int64), _ptr(prof, C.c_uint64),
+                                        _ptr(cons, C.c_char), C.c_int64(cap), C.byref(ncols))
+        rc = load().vsg_cluster_msa(*args(None, None, 0))
+        if rc == -5:   # VSG_ECAP: sized by the first call
+            prof = np.zeros((ncols.value, 6), dtype=np.uint64)
+            cons = np.zeros(ncols.value, dtype=np.uint8)
+            rc = load().vsg_cluster_msa(*args(prof, cons, ncols.value))
+        else:
+            prof = np.zeros((0, 6), dtype=np.uint64)
+            cons = np.zeros(0, dtype=np.uint8)
+        _check(rc, "vsg_cluster_msa")
+        return {"insertions": ins[:nins], "col_first": first, "profile": prof, "consensus": cons}
 
     def exact_index(self, db: SeqSetHandle) -> "ExactIndex":
         """vsg_exact_index_create: the hash index of every sequence of `db` (which must outlive it)"""
@@ -845,8 +876,56 @@ def cluster_cmd_opts(command: str = "cluster_fast", **kw):
     return c, s
 
 
+class ClusterCmdOutputs(C.Structure):
+    _fields_ = [("uc", C.c_char_p), ("centroids", C.c_char_p), ("clusters_prefix", C.c_char_p), ("msaout", C.c_char_p),
+                ("consout", C.c_char_p), ("profile", C.c_char_p)]
+
+
 def _cluster_cmd_paths(uc, centroids, clusters):
     return tuple(p.encode() if p is not None else None for p in (uc, centroids, clusters))
+
+
+def _cigar_buf(cigars, n):
+    """the CIGARs (str, None for S records) back to back, NUL-terminated, and their offsets"""
+    cig = [(x or "").encode() + b"\0" for x in cigars]
+    cbuf = np.frombuffer(b"".join(cig) + b"\0", dtype=np.uint8)
+    coff = np.zeros(max(n, 1), dtype=np.int64)
+    if n > 1:
+        coff[1:n] = np.cumsum([len(x) for x in cig[:-1]], dtype=np.int64)
+    return cbuf, coff
+
+
+def _records(seqs):
+    n = len(seqs)
+    cat = np.frombuffer(b"".join(seqs) + b"\0", dtype=np.uint8)
+    ln = np.array([len(x) for x in seqs], dtype=np.int32)
+    off = np.zeros(n, dtype=np.int64)
+    if n > 1:
+        off[1:] = np.cumsum(ln[:-1], dtype=np.int64)
+    return cat, off, ln
+
+
+def cluster_msa_write(headers, seqs, abundances, results: np.ndarray, cigars, msa: dict, msaout: Optional[str] = None,
+                      consout: Optional[str] = None, profile: Optional[str] = None, command: str = "cluster_fast", **opts):
+    """vsg_cluster_msa_write (host only, no device): --msaout, --consout and --profile of records in processing order
+    (as cluster_write takes them) from `msa`, a dict of cluster_msa's arrays.  opts as cluster_cmd_opts."""
+    c, _ = cluster_cmd_opts(command, **opts)
+    n = len(headers)
+    res = np.ascontiguousarray(results, dtype=_CLUSTER_DT)
+    cat, off, ln = _records(seqs)
+    cbuf, coff = _cigar_buf(cigars, n)
+    ab = np.ascontiguousarray(abundances, dtype=np.int64)
+    ins = np.ascontiguousarray(msa["insertions"], dtype=np.int32)
+    first = np.ascontiguousarray(msa["col_first"], dtype=np.int64)
+    prof = np.ascontiguousarray(msa["profile"], dtype=np.uint64)
+    cons = np.ascontiguousarray(msa["consensus"], dtype=np.uint8)
+    _check(load().vsg_cluster_msa_write(C.c_int64(n), _strings(headers) if n else None, cat.ctypes.data_as(C.c_char_p),
+                                        _ptr(off, C.c_int64), _ptr(ln, C.c_int32), _ptr(ab, C.c_int64),
+                                        res.ctypes.data_as(C.POINTER(ClusterResult)), cbuf.ctypes.data_as(C.c_char_p),
+                                        _ptr(coff, C.c_int64), ins.ctypes.data_as(C.POINTER(C.c_int32)),
+                                        first.ctypes.data_as(C.POINTER(C.c_int64)), prof.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                        cons.ctypes.data_as(C.c_char_p), C.byref(c),
+                                        *_cluster_cmd_paths(msaout, consout, profile)), "vsg_cluster_msa_write")
 
 
 def cluster_write(headers, seqs, abundances, results: np.ndarray, cigars, uc: Optional[str] = None,
@@ -857,16 +936,8 @@ def cluster_write(headers, seqs, abundances, results: np.ndarray, cigars, uc: Op
     c, _ = cluster_cmd_opts(command, **opts)
     n = len(headers)
     res = np.ascontiguousarray(results, dtype=_CLUSTER_DT)
-    cat = np.frombuffer(b"".join(seqs) + b"\0", dtype=np.uint8)
-    ln = np.array([len(x) for x in seqs], dtype=np.int32)
-    off = np.zeros(n, dtype=np.int64)
-    if n > 1:
-        off[1:] = np.cumsum(ln[:-1], dtype=np.int64)
-    cig = [(x or "").encode() + b"\0" for x in cigars]
-    cbuf = np.frombuffer(b"".join(cig) + b"\0", dtype=np.uint8)
-    coff = np.zeros(max(n, 1), dtype=np.int64)
-    if n > 1:
-        coff[1:n] = np.cumsum([len(x) for x in cig[:-1]], dtype=np.int64)
+    cat, off, ln = _records(seqs)
+    cbuf, coff = _cigar_buf(cigars, n)
     ab = np.ascontiguousarray(abundances, dtype=np.int64)
     single = C.c_int64()
     _check(load().vsg_cluster_write(C.c_int64(n), _strings(headers) if n else None, cat.ctypes.data_as(C.c_char_p),
