@@ -819,6 +819,57 @@ int vsg_search_write(int64_t nq, const char * const * query_headers, const char 
                      const int64_t * dboff, const int32_t * dblen, const int64_t * db_sizes, const vsg_usearch_global_opts * u,
                      const vsg_usearch_global_outputs * outputs, int64_t * matched);
 
+/* ---- Chimera detection: the --uchime_ref, --uchime_denovo, --uchime2_denovo and --uchime3_denovo commands
+ *      (core/chimera.cpp), with the output files of `vsearch ... --threads 1`.  Each query of 4 nt or more is cut into
+ *      four pieces that are searched on the device (--id 0.55, maxaccepts 4, maxrejects 16); the whole query is aligned
+ *      with the accepted targets, the two parents are selected on the device, and the parents are evaluated on the host.
+ *      --uchime_ref: the queries (input_path) are FASTA, read and printed as they are (never DUST-masked; with --qmask
+ *      soft or dust their lower case is left out of the k-mer search); the database (db_path) is FASTA (dbmask none,
+ *      soft or dust, --hardmask with soft) or UDB.
+ *      De novo (db_path NULL): the input is FASTA or FASTQ, read as db.read keeps it, DUST-masked (--qmask dust) or
+ *      hardmasked, sorted by abundance, and each sequence is searched against the non-chimeras before it, as the
+ *      reference's single thread does.  The sorted input is cut into abundance bands of at most band_cap sequences, none
+ *      of which can be a parent of another under --abskew; a band is searched on the device against the index as it
+ *      stood at its start, then replayed on the host in order (a query whose candidates change is finished again on its
+ *      own: stats.recomputed).  --abskew 1 or less gives bands of one sequence: exact, but one round trip per sequence.
+ *      The abundance of a sequence comes from ";size=".
+ *      Refused with VSG_EINVAL (message in vsg_last_error, no output file left behind): no output file, --uchime_ref
+ *      without a database or de novo with one, gzip or bzip2 input, FASTQ queries for --uchime_ref, --strand both,
+ *      --hardmask with --qmask dust or --dbmask dust, a missing file, a pair the 16-bit aligner defers (its CIGAR would
+ *      come from nowhere). ---- */
+#define VSG_UCHIME_REF 0
+#define VSG_UCHIME_DENOVO 1
+#define VSG_UCHIME_2_DENOVO 2
+#define VSG_UCHIME_3_DENOVO 3
+typedef struct vsg_uchime_opts {   /* vsg_uchime_opts_default(command, &o) sets the CLI's defaults */
+  int32_t command;                 /* VSG_UCHIME_REF / _DENOVO / _2_DENOVO / _3_DENOVO */
+  double abskew, dn, xn, mindiv, minh;   /* --abskew 2.0 (16.0 for --uchime3_denovo; de novo only), --dn 1.4, --xn 8.0, --mindiv 0.8, --minh 0.28 */
+  int32_t mindiffs;                /* --mindiffs 3 */
+  int32_t qmask, dbmask, hardmask; /* VSG_DBMASK_*: --qmask dust, --dbmask dust (--uchime_ref only); --hardmask */
+  int32_t self, selfid;            /* --uchime_ref: --self (label), --selfid (a piece equal to the target); always on de novo */
+  int32_t strand_both;             /* --strand both: refused */
+  int32_t sizeout, xsize, fasta_score, notrunclabels, uchimeout5;
+  int32_t fasta_width, alignwidth; /* 80, 80; < 1: one line */
+  int64_t minseqlength, maxseqlength;   /* records kept (the database's for --uchime_ref, the input's de novo): 1 .. 50 000 */
+  int64_t batch_queries;           /* --uchime_ref: queries per device batch (< 1: 8 192) */
+  int64_t band_cap;                /* de novo: the most sequences in an abundance band (< 1: 1 024) */
+} vsg_uchime_opts;
+typedef struct vsg_uchime_outputs {   /* NULL: not written */
+  const char * chimeras, * nonchimeras, * borderline, * uchimeout, * uchimealns;
+} vsg_uchime_outputs;
+typedef struct vsg_uchime_stats {
+  int64_t queries, chimeras, nonchimeras, borderline;   /* the reference's stderr summary */
+  int64_t queries_abundance, chimeras_abundance, nonchimeras_abundance, borderline_abundance;
+  int64_t db_sequences;            /* --uchime_ref: database sequences */
+  int64_t candidates;              /* whole-query alignments (distinct accepted targets of the pieces) */
+  int64_t part_pairs;              /* alignments of the part searches */
+  int64_t bands, recomputed;       /* de novo: abundance bands; queries the serial pass finished again */
+  double parse_s, search_s, align_s, parents_s, eval_s, serial_s, write_s, wall_s;
+} vsg_uchime_stats;
+void vsg_uchime_opts_default(int command, vsg_uchime_opts * o);
+int vsg_uchime_command(vsg_ctx * ctx, const char * input_path, const char * db_path, const vsg_uchime_opts * o,
+                       const vsg_uchime_outputs * out, vsg_uchime_stats * st);
+
 #ifdef __cplusplus
 }
 #endif

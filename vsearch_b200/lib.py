@@ -448,6 +448,17 @@ class Context:
                                                  C.byref(st)), "vsg_usearch_global_command")
         return {k: getattr(st, k) for k, _ in UsearchGlobalStats._fields_}
 
+    def uchime(self, input_path: str, db_path: Optional[str] = None, /, **kw) -> dict:
+        """vsg_uchime_command: --uchime_ref with db_path a FASTA or UDB file, de novo (command=UCHIME_DENOVO, _2_ or _3_,
+        or its name) with db_path None.  Keywords naming an output of UCHIME_OUTPUTS give its path, the rest the fields of
+        vsg_uchime_opts (qmask / dbmask may be "none" / "soft" / "dust").
+        Returns the stats as a dict."""
+        o, out = uchime_opts(**kw)
+        st = UchimeStats()
+        _check(load().vsg_uchime_command(self.h, input_path.encode(), None if db_path is None else db_path.encode(), C.byref(o),
+                                         C.byref(out), C.byref(st)), "vsg_uchime_command")
+        return {k: getattr(st, k) for k, _ in UchimeStats._fields_}
+
     def udb_load(self, udb: "Udb"):
         """vsg_udb_load: (SeqSetHandle, IndexHandle, mask_lower) of a parsed UDB file"""
         sh = C.c_void_p(); ih = C.c_void_p(); ml = C.c_int(-1)
@@ -1025,6 +1036,49 @@ def usearch_global_opts(**kw):
         else:
             setattr(s, k, v)
     return u, s, o
+
+
+UCHIME_REF, UCHIME_DENOVO, UCHIME_2_DENOVO, UCHIME_3_DENOVO = 0, 1, 2, 3
+UCHIME_COMMANDS = {"uchime_ref": UCHIME_REF, "uchime_denovo": UCHIME_DENOVO, "uchime2_denovo": UCHIME_2_DENOVO,
+                   "uchime3_denovo": UCHIME_3_DENOVO}
+UCHIME_OUTPUTS = ("chimeras", "nonchimeras", "borderline", "uchimeout", "uchimealns")
+
+
+class UchimeOpts(C.Structure):
+    _fields_ = [("command", C.c_int32), ("abskew", C.c_double), ("dn", C.c_double), ("xn", C.c_double), ("mindiv", C.c_double),
+                ("minh", C.c_double), ("mindiffs", C.c_int32), ("qmask", C.c_int32), ("dbmask", C.c_int32), ("hardmask", C.c_int32),
+                ("self", C.c_int32), ("selfid", C.c_int32), ("strand_both", C.c_int32), ("sizeout", C.c_int32), ("xsize", C.c_int32),
+                ("fasta_score", C.c_int32), ("notrunclabels", C.c_int32), ("uchimeout5", C.c_int32), ("fasta_width", C.c_int32),
+                ("alignwidth", C.c_int32), ("minseqlength", C.c_int64), ("maxseqlength", C.c_int64), ("batch_queries", C.c_int64),
+                ("band_cap", C.c_int64)]
+
+
+class UchimeOutputs(C.Structure):
+    _fields_ = [(k, C.c_char_p) for k in UCHIME_OUTPUTS]
+
+
+class UchimeStats(C.Structure):
+    _fields_ = [(k, C.c_int64) for k in ("queries", "chimeras", "nonchimeras", "borderline", "queries_abundance", "chimeras_abundance",
+                                         "nonchimeras_abundance", "borderline_abundance", "db_sequences", "candidates", "part_pairs",
+                                         "bands", "recomputed")] + \
+               [(k, C.c_double) for k in ("parse_s", "search_s", "align_s", "parents_s", "eval_s", "serial_s", "write_s", "wall_s")]
+
+
+def uchime_opts(command=UCHIME_REF, **kw):
+    """vsg_uchime_opts_default(command), then the given fields: output paths into UchimeOutputs, the rest into
+    vsg_uchime_opts.  Returns (UchimeOpts, UchimeOutputs)."""
+    o, out = UchimeOpts(), UchimeOutputs()
+    command = UCHIME_COMMANDS[command] if isinstance(command, str) else int(command)
+    load().vsg_uchime_opts_default(command, C.byref(o))
+    names = {k for k, _ in UchimeOpts._fields_}
+    for k, v in kw.items():
+        if k in UCHIME_OUTPUTS:
+            setattr(out, k, v.encode() if isinstance(v, str) else v)
+        elif k in names:
+            setattr(o, k, DBMASK[v] if isinstance(v, str) else v)
+        else:
+            raise TypeError(f"uchime: unknown option {k}")
+    return o, out
 
 
 def _packed(seqs):
