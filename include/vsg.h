@@ -836,23 +836,38 @@ int vsg_search_write(int64_t nq, const char * const * query_headers, const char 
  *      Refused with VSG_EINVAL (message in vsg_last_error, no output file left behind): no output file, --uchime_ref
  *      without a database or de novo with one, gzip or bzip2 input, FASTQ queries for --uchime_ref, --strand both,
  *      --hardmask with --qmask dust or --dbmask dust, a missing file, a pair the 16-bit aligner defers (its CIGAR would
- *      come from nowhere). ---- */
+ *      come from nowhere).
+ *      --chimeras_denovo (VSG_CHIMERAS_DENOVO, db_path NULL) is the de novo command for long, high-quality reads
+ *      (find_best_parents_long / eval_parents_long): a query is cut into chimeras_parts parts (0: one per 100 nt, 2 to
+ *      100), its parents are the candidates with the longest indel-free stretches that match within chimeras_diff_pct
+ *      percent, up to chimeras_parents_max of them, each at least chimeras_length_min long, and the query is chimeric when
+ *      two or more parents cover it completely.  Its defaults: --abskew 1.0, --alignwidth 60.  Its sorted input is cut
+ *      into bands of band_cap consecutive reads; a band's earlier members are searched as parents of its later ones on
+ *      the speculation that they are non-chimeric, and the serial pass finishes again a query whose candidates that
+ *      changes (stats.recomputed).  The uchimeout slot takes
+ *      its --tabbedout file (a row per chimera only) and the uchimealns slot its --alnout file; --borderline is refused.
+ *      The four chimeras_* fields must keep their defaults for the other commands. ---- */
 #define VSG_UCHIME_REF 0
 #define VSG_UCHIME_DENOVO 1
 #define VSG_UCHIME_2_DENOVO 2
 #define VSG_UCHIME_3_DENOVO 3
+#define VSG_CHIMERAS_DENOVO 4
 typedef struct vsg_uchime_opts {   /* vsg_uchime_opts_default(command, &o) sets the CLI's defaults */
-  int32_t command;                 /* VSG_UCHIME_REF / _DENOVO / _2_DENOVO / _3_DENOVO */
-  double abskew, dn, xn, mindiv, minh;   /* --abskew 2.0 (16.0 for --uchime3_denovo; de novo only), --dn 1.4, --xn 8.0, --mindiv 0.8, --minh 0.28 */
+  int32_t command;                 /* VSG_UCHIME_REF / _DENOVO / _2_DENOVO / _3_DENOVO, VSG_CHIMERAS_DENOVO */
+  double abskew, dn, xn, mindiv, minh;   /* --abskew 2.0 (16.0 for --uchime3_denovo, 1.0 for --chimeras_denovo; de novo only), --dn 1.4, --xn 8.0, --mindiv 0.8, --minh 0.28 */
   int32_t mindiffs;                /* --mindiffs 3 */
   int32_t qmask, dbmask, hardmask; /* VSG_DBMASK_*: --qmask dust, --dbmask dust (--uchime_ref only); --hardmask */
   int32_t self, selfid;            /* --uchime_ref: --self (label), --selfid (a piece equal to the target); always on de novo */
   int32_t strand_both;             /* --strand both: refused */
   int32_t sizeout, xsize, fasta_score, notrunclabels, uchimeout5;
-  int32_t fasta_width, alignwidth; /* 80, 80; < 1: one line */
+  int32_t fasta_width, alignwidth; /* 80, 80 (60 for --chimeras_denovo); < 1: one line */
   int64_t minseqlength, maxseqlength;   /* records kept (the database's for --uchime_ref, the input's de novo): 1 .. 50 000 */
   int64_t batch_queries;           /* --uchime_ref: queries per device batch (< 1: 8 192) */
   int64_t band_cap;                /* de novo: the most sequences in an abundance band (< 1: 1 024) */
+  int32_t chimeras_parts;          /* --chimeras_parts: 0 = (length + 99) / 100, clamped to 2 .. 100; else 2 .. 100 */
+  int32_t chimeras_parents_max;    /* --chimeras_parents_max 3: 2 .. 20 */
+  int32_t chimeras_length_min;     /* --chimeras_length_min 10: at least 1 */
+  double chimeras_diff_pct;        /* --chimeras_diff_pct 0.0: 0 .. 50 */
 } vsg_uchime_opts;
 typedef struct vsg_uchime_outputs {   /* NULL: not written */
   const char * chimeras, * nonchimeras, * borderline, * uchimeout, * uchimealns;

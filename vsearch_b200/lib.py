@@ -449,7 +449,7 @@ class Context:
         return {k: getattr(st, k) for k, _ in UsearchGlobalStats._fields_}
 
     def uchime(self, input_path: str, db_path: Optional[str] = None, /, **kw) -> dict:
-        """vsg_uchime_command: --uchime_ref with db_path a FASTA or UDB file, de novo (command=UCHIME_DENOVO, _2_ or _3_,
+        """vsg_uchime_command: --uchime_ref with db_path a FASTA or UDB file, de novo (command=UCHIME_DENOVO, _2_, _3_ or CHIMERAS_DENOVO,
         or its name) with db_path None.  Keywords naming an output of UCHIME_OUTPUTS give its path, the rest the fields of
         vsg_uchime_opts (qmask / dbmask may be "none" / "soft" / "dust").
         Returns the stats as a dict."""
@@ -1038,9 +1038,9 @@ def usearch_global_opts(**kw):
     return u, s, o
 
 
-UCHIME_REF, UCHIME_DENOVO, UCHIME_2_DENOVO, UCHIME_3_DENOVO = 0, 1, 2, 3
+UCHIME_REF, UCHIME_DENOVO, UCHIME_2_DENOVO, UCHIME_3_DENOVO, CHIMERAS_DENOVO = 0, 1, 2, 3, 4
 UCHIME_COMMANDS = {"uchime_ref": UCHIME_REF, "uchime_denovo": UCHIME_DENOVO, "uchime2_denovo": UCHIME_2_DENOVO,
-                   "uchime3_denovo": UCHIME_3_DENOVO}
+                   "uchime3_denovo": UCHIME_3_DENOVO, "chimeras_denovo": CHIMERAS_DENOVO}
 UCHIME_OUTPUTS = ("chimeras", "nonchimeras", "borderline", "uchimeout", "uchimealns")
 
 
@@ -1050,7 +1050,8 @@ class UchimeOpts(C.Structure):
                 ("self", C.c_int32), ("selfid", C.c_int32), ("strand_both", C.c_int32), ("sizeout", C.c_int32), ("xsize", C.c_int32),
                 ("fasta_score", C.c_int32), ("notrunclabels", C.c_int32), ("uchimeout5", C.c_int32), ("fasta_width", C.c_int32),
                 ("alignwidth", C.c_int32), ("minseqlength", C.c_int64), ("maxseqlength", C.c_int64), ("batch_queries", C.c_int64),
-                ("band_cap", C.c_int64)]
+                ("band_cap", C.c_int64), ("chimeras_parts", C.c_int32), ("chimeras_parents_max", C.c_int32),
+                ("chimeras_length_min", C.c_int32), ("chimeras_diff_pct", C.c_double)]
 
 
 class UchimeOutputs(C.Structure):
