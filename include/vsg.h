@@ -188,6 +188,11 @@ void vsg_index_destroy(vsg_index * ix);
 int vsg_rank(vsg_ctx * ctx, const vsg_index * ix, const vsg_seqset * queries, int64_t q0,
              int64_t nq, int minwordmatches, int tophits, int mask_lower,
              uint32_t * cand_seqno, uint32_t * cand_count, int32_t * ncand);
+/* CTAs per SM the device holds of the ranker's two instances (cudaOccupancyMaxActiveBlocksPerMultiprocessor): the
+ * full one, and the short-query one that vsg_rank and vsg_search_batch use when tophits <= 64 and every query of the
+ * call has np2 + nwin + 1 <= 512 (nwin: its k-mer windows; np2: nwin rounded up to a power of two; at wordlength 8,
+ * queries of up to 262 nt). */
+int vsg_rank_occupancy(vsg_ctx * ctx, int * ctas_full, int * ctas_short);
 
 /* ---- whole-path search: replaces search_batch (core/search.hpp:135-145, search.cpp:511-593) /
  *      the body of search_thread_run (commands/usearch_global.cpp:376-497) for plus-strand (and

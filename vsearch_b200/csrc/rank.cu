@@ -33,9 +33,7 @@
 
 namespace vsg {
 
-constexpr int CAND_CAP = 2048;          // candidate keys held in shared memory
 constexpr int TOPHITS_MAX = RANK_TOPHITS_MAX;
-constexpr int SCAN_SEG_WORDS = 512;     // counters are scanned 1024 at a time (<= 1024 new candidates)
 
 // ---- index build: pass 1 counts, pass 2 fills; one CTA per target, shared-memory bitmap dedupe ----
 template <bool FILL>
@@ -239,11 +237,12 @@ __device__ __forceinline__ int threshold_from_hist(const uint32_t * hist, int to
   return floor;
 }
 
-// Compacts the keys >= tkey of cand[0, m) in place to its front (in no order) and returns how many there are.  Every
-// thread reads its keys before any is written back.
+// Compacts the keys >= tkey of cand[0, m) (m <= CAND) in place to its front (in no order) and returns how many there
+// are.  Every thread reads its keys before any is written back.
+template <int CAND>
 __device__ __forceinline__ int keep_keys_from(uint64_t * cand, int m, uint64_t tkey, int & s_ncand)
 {
-  uint64_t mine[CAND_CAP / RANK_THREADS];
+  uint64_t mine[(CAND + RANK_THREADS - 1) / RANK_THREADS];
   int cnt = 0;
   for (int i = threadIdx.x; i < m; i += blockDim.x) { uint64_t const kx = cand[i]; if (kx >= tkey) { mine[cnt++] = kx; } }
   if (threadIdx.x == 0) { s_ncand = 0; }
@@ -357,8 +356,26 @@ __device__ __forceinline__ void postings_incr(const ShardDev & S, int n, const u
 // each query reach the reference's threshold, RANK_EMIT writes their keys to keys[key_off[qi] ...] in no order.
 enum { RANK_TOP = 0, RANK_COUNT = 1, RANK_EMIT = 2 };
 
-template <bool INCR, int MODE = RANK_TOP>
-__global__ void __launch_bounds__(RANK_THREADS, 2)
+// The shapes rank_kernel is compiled for, both of RANK_THREADS threads: CTAS per SM (the register bound of
+// __launch_bounds__), KCAP k-mer slots per query, CAND candidate keys and SEG counter words per segment of the sort-and-cut scan (each
+// segment appends at most 2 * SEG keys, so tophits + 2 * SEG <= CAND must hold).
+//   RankFull: every mode and both indexes; queries of up to KCAP windows in shared memory, longer ones through HBM
+//     scratch.  114 708 B of shared memory: two CTAs per SM.
+//   RankShort: RANK_TOP on the static index with tophits <= 64, every query of the launch with np2 + nwin + 1 <= 512
+//     (so its k-mers and the running threshold's histogram fit the k-mer array: at wordlength 8, queries of up to
+//     262 nt).  75 796 B of shared memory and <= 40 registers (ptxas: 40, and 36 B of spill stores, none of them in
+//     postings_stream's loop, whose code matches RankFull's): three CTAs per SM, 1.5x the posting loads in flight of
+//     RankFull.  (256-thread CTAs with 8 vectors per lane would allow 80 registers; at 40 nothing in the loop spills.)
+struct RankFull { static constexpr int CTAS = 2, KCAP = KMER_CAP, CAND = 2048, SEG = 512; };
+struct RankShort { static constexpr int CTAS = 3, KCAP = 512, CAND = 256, SEG = 64, TOPHITS = 64; };
+
+template <typename CFG>
+constexpr size_t rank_smem() { return CFG::CAND * 8 + (COUNTER_WORDS + 3) * 4 + CFG::KCAP * 4 * 4 + 4; }
+static_assert(rank_smem<RankFull>() == 114708 && rank_smem<RankShort>() == 75796, "rank_kernel's shared memory");
+static_assert(RankShort::TOPHITS + 2 * RankShort::SEG <= RankShort::CAND, "a sort-and-cut segment must fit behind tophits keys");
+
+template <typename CFG, bool INCR, int MODE = RANK_TOP>
+__global__ void __launch_bounds__(RANK_THREADS, CFG::CTAS)
 rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restrict__ shards, int nshards,
             int k, int mask_lower, int minwordmatches, int tophits,
             uint32_t * __restrict__ out_seqno, uint32_t * __restrict__ out_count, int32_t * __restrict__ out_n,
@@ -366,12 +383,13 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
             const int64_t * __restrict__ key_off, uint64_t * __restrict__ keys)
 {
   extern __shared__ __align__(16) unsigned char smem[];
-  uint64_t * const cand = reinterpret_cast<uint64_t *>(smem);                     // CAND_CAP
-  uint32_t * const counters = reinterpret_cast<uint32_t *>(smem + CAND_CAP * 8);  // COUNTER_WORDS (+pad)
-  uint32_t * const kmers = counters + COUNTER_WORDS + 3;                          // KMER_CAP
-  uint32_t * const lbeg = kmers + KMER_CAP;                                       // KMER_CAP
-  uint32_t * const llen = lbeg + KMER_CAP;                                        // KMER_CAP
-  uint32_t * const cum = llen + KMER_CAP;                                         // KMER_CAP + 1 (static index, flat stream)
+  constexpr int KCAP = CFG::KCAP, CAND = CFG::CAND, SEG = CFG::SEG;
+  uint64_t * const cand = reinterpret_cast<uint64_t *>(smem);                 // CAND
+  uint32_t * const counters = reinterpret_cast<uint32_t *>(smem + CAND * 8);  // COUNTER_WORDS (+pad)
+  uint32_t * const kmers = counters + COUNTER_WORDS + 3;                      // KCAP
+  uint32_t * const lbeg = kmers + KCAP;                                       // KCAP
+  uint32_t * const llen = lbeg + KCAP;                                        // KCAP
+  uint32_t * const cum = llen + KCAP;                                         // KCAP + 1 (static index, flat stream)
   __shared__ int s_ncand, s_nk, s_T, s_K;
   __shared__ int s_wsum[RANK_THREADS / 32];
 
@@ -384,12 +402,12 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
     int const len = qs.len[q];
     int const nwin = len - k + 1;
     if (threadIdx.x == 0) { s_ncand = 0; s_nk = 0; }
-    bool const longq = nwin > KMER_CAP;
+    bool const longq = nwin > KCAP;
     if (longq && (scratch == nullptr || nwin > 65535)) {
       if (threadIdx.x == 0) { out_n[qi] = 0; atomicExch(status, 1); }
       continue;
     }
-    // 1. the query's distinct k-mers: in shared memory, or in HBM scratch, fed through shared memory KMER_CAP at a time
+    // 1. the query's distinct k-mers: in shared memory, or in HBM scratch, fed through shared memory KCAP at a time
     int np2, nk, nchunks = 1;
     uint32_t * gk = nullptr;
     if (!longq) {
@@ -398,17 +416,17 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
       uint32_t * const bm = scratch + static_cast<size_t>(blockIdx.x) * scratch_stride;
       gk = bm + bitmap_words;
       nk = query_kmers_hbm(s, nwin, k, mask_lower, bm, bitmap_words, gk, s_nk);
-      nchunks = nk > 0 ? (nk + KMER_CAP - 1) / KMER_CAP : 1;
+      nchunks = nk > 0 ? (nk + KCAP - 1) / KCAP : 1;
       np2 = 1;
     }
     // search_topscores: count >= min(minwordmatches, kmersamplecount)  (searchcore.cpp:320)
     uint32_t const minmatches = static_cast<uint32_t>(minwordmatches < nk ? minwordmatches : nk);
-    // RUNNING THRESHOLD (queries with np2 + nk + 1 <= KMER_CAP, i.e. up to ~1000 nt): hist[c] counts,
+    // RUNNING THRESHOLD (queries with np2 + nk + 1 <= KCAP, i.e. up to ~1000 nt in RankFull): hist[c] counts,
     // over the shards seen so far, the targets whose k-mer count is c; T = the largest count with at
     // least `tophits` targets at or above it.  A target below T can never reach the final list, so
     // only counts >= T are turned into candidate keys: a few dozen per shard instead of the ~3 % of
     // all targets that pass the reference's fixed threshold (searchcore.cpp:320), no overflow sorts.
-    bool const running = MODE == RANK_TOP && !longq && (np2 + nk + 1 <= KMER_CAP);
+    bool const running = MODE == RANK_TOP && !longq && (np2 + nk + 1 <= KCAP);
     uint32_t * const hist = kmers + np2;  // nk + 1 bins in the unused tail of the k-mer array
     if (running) {
       for (int i = threadIdx.x; i <= nk; i += blockDim.x) { hist[i] = 0; }
@@ -422,15 +440,15 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
       clean = false;
       for (int chunk = 0; chunk < nchunks; chunk++) {
         if (longq) {
-          int const cn = nk > 0 ? min(KMER_CAP, nk - chunk * KMER_CAP) : 1;
-          for (int i = threadIdx.x; i < cn; i += blockDim.x) { kmers[i] = nk > 0 ? gk[chunk * KMER_CAP + i] : 0xffffffffu; }
+          int const cn = nk > 0 ? min(KCAP, nk - chunk * KCAP) : 1;
+          for (int i = threadIdx.x; i < cn; i += blockDim.x) { kmers[i] = nk > 0 ? gk[chunk * KCAP + i] : 0xffffffffu; }
           np2 = cn;
           __syncthreads();
         }
         list_bounds<INCR>(S, kmers, np2, lbeg, llen);
         __syncthreads();
         if constexpr (INCR) { postings_incr(S, np2, lbeg, llen, counters); }
-        else { postings_stream(S, np2, lbeg, llen, cum, counters, s_wsum); }
+        else { postings_stream<KCAP>(S, np2, lbeg, llen, cum, counters, s_wsum); }
         __syncthreads();
       }
       // 4. collect this shard's candidates
@@ -459,7 +477,7 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
         int const level = s_ncand;
         __syncthreads();
         uint32_t const T1 = static_cast<uint32_t>(s_T);
-        if (level + s_K <= CAND_CAP) {
+        if (level + s_K <= CAND) {
           // at most K targets (all shards so far) are >= T1, so at most K keys are appended here
           visit_counters<4>(counters, 0, nwords, S.nt, T1, true, [&](uint32_t c, int lt) {
             cand[atomicAdd(&s_ncand, 1)] = target_key(db, S, c, lt);
@@ -478,7 +496,7 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
         int pos = block_exclusive_sum(mine, s_wsum, total);
         int const level = s_ncand;
         __syncthreads();
-        if (level + total <= CAND_CAP) {
+        if (level + total <= CAND) {
           pos += level;
           visit_counters<1>(counters, 0, nwords, S.nt, minmatches, false, [&](uint32_t c, int lt) {
             cand[pos++] = target_key(db, S, c, lt);
@@ -489,17 +507,17 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
         }
       }
       // 4b. segmented scan with sort-and-cut when the candidate list could overflow
-      for (int seg = 0; seg < nwords; seg += SCAN_SEG_WORDS) {
+      for (int seg = 0; seg < nwords; seg += SEG) {
         // every thread must take the same decision: read the fill level, then fence the read off
         // from the appends of threads that are already past this point
         int const level = s_ncand;
         __syncthreads();
-        if (level + 2 * SCAN_SEG_WORDS > CAND_CAP) {
+        if (level + 2 * SEG > CAND) {
           int const nkeep = sort_and_cut(cand, level, tophits);
           if (threadIdx.x == 0) { s_ncand = nkeep; }
           __syncthreads();
         }
-        visit_counters<1>(counters, seg, min(seg + SCAN_SEG_WORDS, nwords), S.nt, thr, false, [&](uint32_t c, int lt) {
+        visit_counters<1>(counters, seg, min(seg + SEG, nwords), S.nt, thr, false, [&](uint32_t c, int lt) {
           cand[atomicAdd(&s_ncand, 1)] = target_key(db, S, c, lt);
         });
         __syncthreads();
@@ -512,12 +530,12 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
       continue;  // next query
     }
     // Usually far more targets pass the k-mer threshold than are wanted: find the count T of the tophits-th best,
-    // keep count >= T, sort only those.  (A running query has nk < KMER_CAP and its T already.)
+    // keep count >= T, sort only those.  (A running query has nk < KCAP and its T already.)
     int m = s_ncand;
     __syncthreads();
-    if (m > 2 * tophits && nk + 1 <= 2 * KMER_CAP) {
+    if (m > 2 * tophits && nk + 1 <= 2 * KCAP) {
       if (!running) {
-        uint32_t * const hist5 = lbeg;  // 2 * KMER_CAP words available, counts are <= nk
+        uint32_t * const hist5 = lbeg;  // 2 * KCAP words available, counts are <= nk
         for (int i = threadIdx.x; i <= nk; i += blockDim.x) { hist5[i] = 0; }
         __syncthreads();
         for (int i = threadIdx.x; i < m; i += blockDim.x) { atomicAdd(&hist5[static_cast<uint32_t>(cand[i] >> 49)], 1u); }
@@ -530,7 +548,7 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
         __syncthreads();
       }
       // running: the keys below the final T were appended while T was still lower
-      m = keep_keys_from(cand, m, count_key(s_T), s_ncand);
+      m = keep_keys_from<CAND>(cand, m, count_key(s_T), s_ncand);
     }
     int const nout = sort_and_cut(cand, m, tophits);
     for (int i = threadIdx.x; i < nout; i += blockDim.x) {
@@ -543,7 +561,6 @@ rank_kernel(DevSeqs qs, int64_t q0, int nq, DevSeqs db, const ShardDev * __restr
   }
 }
 
-constexpr size_t RANK_SMEM = CAND_CAP * 8 + (COUNTER_WORDS + 3) * 4 + KMER_CAP * 4 * 4 + 4;   // 114 708 B: two CTAs fit an SM's 227 KB
 
 }  // namespace vsg
 
@@ -886,23 +903,37 @@ RankTargets index_targets(const vsg_index * ix, int mask_lower)
   return t;
 }
 
-// Launches rank_kernel<t.incr, MODE> on c's stream over queries [q0, q0 + nq) (nq >= 1) against t's shards: two CTAs per
-// SM at most, and HBM scratch when a query has more than KMER_CAP windows.  t.timed: ev[4..5] around the launch, added
-// to vsg_profile.rank_ms by rank_collect_time.
+// Whether rank_kernel<RankShort> can rank a launch of RANK_TOP on the static index whose longest query has maxlen nt:
+// every query's np2 + nwin + 1 must fit RankShort::KCAP, and np2 + nwin grows with the length.
+static bool rank_short_fits(bool incr, int tophits, int maxlen, int k)
+{
+  int const nwin = std::max(1, maxlen - k + 1);
+  int np2 = 1;
+  while (np2 < nwin) { np2 <<= 1; }
+  return !incr && tophits <= RankShort::TOPHITS && np2 + nwin + 1 <= RankShort::KCAP;
+}
+
+// Launches rank_kernel on c's stream over queries [q0, q0 + nq) (nq >= 1) against t's shards: rank_kernel<RankShort>
+// (three CTAs per SM) when rank_short_fits, else rank_kernel<RankFull, t.incr, MODE> (two CTAs per SM) with HBM
+// scratch when a query has more than KMER_CAP windows.  t.timed: ev[4..5] around the launch, added to
+// vsg_profile.rank_ms by rank_collect_time.
 template <int MODE>
 static int rank_launch(vsg_ctx * c, const RankTargets & t, const vsg_seqset * queries, int64_t q0, int64_t nq,
                        int minwordmatches, int tophits, const RankTop & out, const int64_t * d_key_off, uint64_t * d_keys)
 {
   int rc;
-  auto const kernel = t.incr ? rank_kernel<true, MODE> : rank_kernel<false, MODE>;
   int const k = t.k;
-  VSG_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(RANK_SMEM)));
-  int sms = 132;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
-  int const grid = static_cast<int>(std::min<int64_t>(nq, static_cast<int64_t>(sms) * 2));
-  // queries with more than KMER_CAP windows de-duplicate their k-mers in HBM scratch
   int maxlen = 0;
   for (int64_t q = q0; q < q0 + nq; q++) { maxlen = std::max(maxlen, queries->h_len[static_cast<size_t>(q)]); }
+  bool const small = MODE == RANK_TOP && rank_short_fits(t.incr, tophits, maxlen, k);
+  auto const kernel = small ? rank_kernel<RankShort, false, RANK_TOP>
+                            : t.incr ? rank_kernel<RankFull, true, MODE> : rank_kernel<RankFull, false, MODE>;
+  size_t const smem = small ? rank_smem<RankShort>() : rank_smem<RankFull>();
+  VSG_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  int sms = 132;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+  int const grid = static_cast<int>(std::min<int64_t>(nq, static_cast<int64_t>(sms) * (small ? RankShort::CTAS : RankFull::CTAS)));
+  // queries with more than KMER_CAP windows de-duplicate their k-mers in HBM scratch
   uint32_t * d_scratch = nullptr;
   size_t stride = 0;
   int bitmap_words = std::max(1, (1 << (2 * std::min(k, 10))) >> 5);
@@ -913,7 +944,7 @@ static int rank_launch(vsg_ctx * c, const RankTargets & t, const vsg_seqset * qu
     d_scratch = static_cast<uint32_t *>(c->rank_scratch.p);
   }
   if (t.timed) { VSG_CUDA_OK(cudaEventRecord(c->ev[4], c->stream)); }
-  kernel<<<grid, RANK_THREADS, RANK_SMEM, c->stream>>>(
+  kernel<<<grid, RANK_THREADS, smem, c->stream>>>(
       queries->d, q0, static_cast<int>(nq), t.lens, t.shards, t.nshards, k, t.mask_lower, minwordmatches, tophits,
       out.seqno, out.count, out.n, out.status, d_scratch, stride, bitmap_words, d_key_off, d_keys);
   count_launch();
@@ -1089,6 +1120,19 @@ extern "C" int vsg_rank(vsg_ctx * c, const vsg_index * ix, const vsg_seqset * qu
   if (rc == VSG_OK) { rc = rank_download(c, r, nq, tophits, cand_seqno, cand_count, ncand, "vsg_rank"); }
   if (rc != VSG_OK) { return rc; }
   VSG_CUDA_OK(cudaGetLastError());
+  return VSG_OK;
+}
+
+extern "C" int vsg_rank_occupancy(vsg_ctx * c, int * ctas_full, int * ctas_short)
+{
+  if (c == nullptr || ctas_full == nullptr || ctas_short == nullptr) { Error::set("vsg_rank_occupancy: null argument"); return VSG_EINVAL; }
+  VSG_CUDA_OK(cudaSetDevice(c->device));
+  auto const full = rank_kernel<RankFull, false, RANK_TOP>;
+  auto const small = rank_kernel<RankShort, false, RANK_TOP>;
+  VSG_CUDA_OK(cudaFuncSetAttribute(full, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(rank_smem<RankFull>())));
+  VSG_CUDA_OK(cudaFuncSetAttribute(small, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(rank_smem<RankShort>())));
+  VSG_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_full, full, RANK_THREADS, rank_smem<RankFull>()));
+  VSG_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_short, small, RANK_THREADS, rank_smem<RankShort>()));
   return VSG_OK;
 }
 

@@ -154,7 +154,9 @@ __device__ __forceinline__ void list_bounds(const ShardDev & S, const uint32_t *
 //      lbeg[i] = first vector - c_i  so that stream position + lbeg = the vector's index in the shard's postings
 //      llen[i] = c_i + na_i         positions below it hold even targets (increment 1), the rest odd ones (0x10000)
 //    A lane finds its first run by one binary search and then walks forward (runs average two rounds).
-//    llen and cum must lie KMER_CAP and 2 * KMER_CAP words behind lbeg: the walk addresses them from lbeg.
+//    KCAP: the capacity of the run arrays (n <= KCAP); llen and cum must lie KCAP and 2 * KCAP words behind lbeg: the
+//    walk addresses them from lbeg.
+template <int KCAP = KMER_CAP>
 __device__ __forceinline__ void postings_stream(const ShardDev & S, int n, uint32_t * lbeg, uint32_t * llen, uint32_t * cum,
                                                 uint32_t * counters, int * s_wsum)
 {
@@ -163,12 +165,12 @@ __device__ __forceinline__ void postings_stream(const ShardDev & S, int n, uint3
   uint32_t Vtot;
   {
     // 3a. exclusive prefix sum of the run lengths (in vectors)
-    int const per = (n + RANK_THREADS - 1) / RANK_THREADS;   // <= 4
+    int const per = (n + RANK_THREADS - 1) / RANK_THREADS;   // <= KCAP / RANK_THREADS
     int const i0 = threadIdx.x * per;
-    uint32_t nn[KMER_CAP / RANK_THREADS], bb[KMER_CAP / RANK_THREADS];
+    uint32_t nn[KCAP / RANK_THREADS], bb[KCAP / RANK_THREADS];
     uint32_t sum = 0;
 #pragma unroll
-    for (int u = 0; u < KMER_CAP / RANK_THREADS; u++) {
+    for (int u = 0; u < KCAP / RANK_THREADS; u++) {
       bool const in = u < per && i0 + u < n;
       nn[u] = in ? llen[i0 + u] : 0u;
       bb[u] = in ? lbeg[i0 + u] : 0u;
@@ -176,7 +178,7 @@ __device__ __forceinline__ void postings_stream(const ShardDev & S, int n, uint3
     }
     uint32_t c0 = block_exclusive_sum(sum, s_wsum, Vtot);
 #pragma unroll
-    for (int u = 0; u < KMER_CAP / RANK_THREADS; u++) {
+    for (int u = 0; u < KCAP / RANK_THREADS; u++) {
       if (u < per && i0 + u < n) {
         uint32_t const na = nn[u] & 0xffffu, nv = na + (nn[u] >> 16);
         lbeg[i0 + u] = (bb[u] >> 3) - c0;
@@ -201,7 +203,7 @@ __device__ __forceinline__ void postings_stream(const ShardDev & S, int n, uint3
       int const mid = (lo + hi) >> 1;
       if (cum[mid] <= v_first) { lo = mid + 1; } else { hi = mid; }
     }
-    // sa walks the run arrays as a shared-memory byte address of lbeg[s]; llen and cum lie KMER_CAP words further each
+    // sa walks the run arrays as a shared-memory byte address of lbeg[s]; llen and cum lie KCAP words further each
     uint32_t sa = static_cast<uint32_t>(__cvta_generic_to_shared(lbeg + lo));
     uint32_t ce = cum[lo];
     // U loads per lane are issued back to back, then turned into counter updates; the other 31 warps of the SM
@@ -213,11 +215,11 @@ __device__ __forceinline__ void postings_stream(const ShardDev & S, int n, uint3
       if (vv < wend) {
         while (vv >= ce) {
           sa += 4u;
-          asm("ld.shared.u32 %0, [%1+%2];" : "=r"(ce) : "r"(sa), "n"(2 * KMER_CAP * 4));
+          asm("ld.shared.u32 %0, [%1+%2];" : "=r"(ce) : "r"(sa), "n"(2 * KCAP * 4));
         }
         uint32_t vb, sp;
         asm("ld.shared.u32 %0, [%1];" : "=r"(vb) : "r"(sa));
-        asm("ld.shared.u32 %0, [%1+%2];" : "=r"(sp) : "r"(sa), "n"(KMER_CAP * 4));
+        asm("ld.shared.u32 %0, [%1+%2];" : "=r"(sp) : "r"(sa), "n"(KCAP * 4));
         cur[u] = __ldg(pbase + static_cast<uint32_t>(vb + vv));
         inc[u] = vv < sp ? 1u : 0x10000u;
       }

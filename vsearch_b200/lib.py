@@ -476,6 +476,12 @@ class Context:
                                _ptr(count, C.c_uint32), _ptr(nc, C.c_int32)), "vsg_rank")
         return seqno, count, nc
 
+    def rank_occupancy(self):
+        """(full, short): CTAs per SM of the ranker's full and short-query instances"""
+        full = C.c_int(); short = C.c_int()
+        _check(load().vsg_rank_occupancy(self.h, C.byref(full), C.byref(short)), "vsg_rank_occupancy")
+        return full.value, short.value
+
     def sintax(self, ix: IndexHandle, qs: SeqSetHandle, q0: int, nq: int, seed: int, strand_both: int = 0,
                query_number0: Optional[int] = None, random_ties: int = 0):
         """vsg_sintax -> dict of numpy arrays: strand[nq], nboot[nq, 2], best_count[nq, 2], seqno[nq, 2, 100] (-1 beyond
